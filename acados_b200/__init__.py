@@ -1,4 +1,4 @@
-"""acados_b200 -- B200-native batched OCP-QP interior-point solver (cuipm) behind acados' ocp_qp plugin surface.
+"""acados_b200 -- H100-native batched OCP-QP interior-point solver (cuipm) behind acados' ocp_qp plugin surface.
 
 Only what the hot path needs lives here: ``csrc/`` (CUDA kernels + the C ABI of include/cuipm.h),
 ``plugin/`` (the plain-C acados qp_solver plugin that calls the C ABI), ``binding`` (ctypes), ``problems``

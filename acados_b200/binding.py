@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI in ``include/cuipm.h`` (libcuipm.so, built in-tree by ``__graft_entry__.build``).
 
-The library is the product: hand-written sm_100a CUDA kernels behind plain-C entry points.  There is no
+The library is the product: hand-written sm_90a CUDA kernels behind plain-C entry points.  There is no
 CPU fallback -- if the shared object is missing, or no CUDA device is present, the solve calls raise.
 """
 from __future__ import annotations

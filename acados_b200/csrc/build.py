@@ -1,4 +1,4 @@
-"""In-tree build of libcuipm.so (CUDA kernels for sm_100a + the C ABI of include/cuipm.h).
+"""In-tree build of libcuipm.so (CUDA kernels for sm_90a + the C ABI of include/cuipm.h).
 
 ``python -m acados_b200.csrc.build [--force] [--verbose]``; also called by ``__graft_entry__.build()``.
 nvcc cross-compiles without a GPU.  Objects are cached under csrc/build/ keyed by source mtime.
@@ -15,7 +15,7 @@ OUT = os.path.join(HERE, "libcuipm.so")
 SOURCES = ["cuipm_kernel.cu", "cuipm_fast.cu", "cuipm_api.cu", "cuipm_reduce.cu", "cuipm_condense.cu", "cuipm_xcond.cu", "cuipm_host.cpp"]
 HEADERS = ["cuipm_device.h", "cuipm_internal.h", "cuipm_plan.h", "cuipm_fast_core.h", "cuipm_condense_core.h", "cuipm_condense_plan.h", os.path.join(ROOT, "include", "cuipm.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
          "-I" + os.path.join(ROOT, "include"), "-I" + HERE]
 if os.environ.get("CUIPM_PROFILE"):
     FLAGS.append("-DCUIPM_PROFILE")   # per-pass cycle counters into the last row of the stat table (development)

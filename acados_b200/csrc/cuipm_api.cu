@@ -124,9 +124,7 @@ static int launch_batch(cuipm_solver *s, const LaunchArgs &a0, int slot, size_t 
         (*launches)++;
         if (slot == 0 && s->evk0) cudaEventRecord(s->evk0, stream);
         // iteration-sliced scheduling pays when the batch is more than one wave of resident QPs and not many; small batches keep the
-        // single launch
-        // (measured on the headline shape: 4096 QPs on 2368 resident ones 89 k -> 99 k QP/s, 8192: 92 k -> 110 k; 2048, less
-        // than one wave: 80 k -> 73 k)
+        // single launch (below one wave the extra launch and the ring traffic cost more than the idle slots they save)
         if (s->rr_ok && s->rr_resident == 0) s->rr_resident = fast_resident_qps(F) > 0 ? fast_resident_qps(F) : -1;
         const bool rr = s->rr_ok && s->use_rr && (s->use_rr > 1 || (s->rr_resident > 0 && a.nbatch > s->rr_resident));
         if (rr)

@@ -1,4 +1,4 @@
-// cuipm_fast.cu -- CUDA instantiation (sm_100a) of the throughput kernel of the batched OCP-QP interior-point solver.
+// cuipm_fast.cu -- CUDA instantiation (sm_90a) of the throughput kernel of the batched OCP-QP interior-point solver.
 //
 // The kernel body is cuipm_fast_core.h (a group of G lanes per QP, 32/G QPs per warp in lock step, register-tiled
 // rank-k updates, stage blocks staged with asynchronous copies); this file binds its warp primitives to the hardware
@@ -267,7 +267,15 @@ bool fast_available(int nx, int nu, FastArgs &F, int *qp_per_warp)
 int launch_repack(const FastArgs &F, const StageDesc *sd, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t) stream_;
-    const int grid = F.nbatch < 148 * 8 ? F.nbatch : 148 * 8;
+    static int sms = 0;
+    if (!sms)
+    {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        if (sms <= 0) sms = 1;
+    }
+    const int grid = F.nbatch < sms * 8 ? F.nbatch : sms * 8;      // eight CTAs per SM, grid-stride over the batch
     cuipm_repack_kernel<<<grid, 256, 0, stream>>>(F, sd);
     return (int) cudaGetLastError();
 }

@@ -23,7 +23,7 @@
 //
 // Scheduling: either a group keeps its QP for the whole solve (run / solve), or -- batches larger than the QPs the device holds
 // at once -- for one iteration at a time, the unfinished QPs circulating through rings ordered by their duality measure
-// (rr_first / rr_loop below: same arithmetic, bit-identical results, 30 % more throughput on the headline batch).  For one QP per
+// (rr_first / rr_loop below: same arithmetic, bit-identical results, fewer idle slots at the end of the headline batch).  For one QP per
 // warp and contraction lengths that are multiples of four the level-3 parts of the factorisation run on the FP64 tensor cores
 // (fk_dmma: mma.m8n8k4), otherwise on register tiles.
 //
@@ -50,7 +50,7 @@
 
 // The short loops of a lane over its elements of a vector (run-time trip counts of 1..4) are kept as loops: the compiler's
 // unroll-by-four with a remainder chain executes more instructions than the loop it replaces at these trip counts, and
-// multiplies the instruction footprint of the sweeps (measured on the headline shape: 76.5k -> 88.4k QP/s, SASS 574 -> 337 KB).
+// multiplies the instruction footprint of the sweeps (on the headline shape the SASS shrinks from 574 to 337 KB).
 #define FK_PRAGMA_(x) _Pragma(#x)
 #define FK_PRAGMA(x) FK_PRAGMA_(x)
 #ifndef FK_VLOOP_N

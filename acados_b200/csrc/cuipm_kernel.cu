@@ -1,4 +1,4 @@
-// cuipm_kernel.cu -- the batched OCP-QP interior-point kernel (sm_100a).
+// cuipm_kernel.cu -- the batched OCP-QP interior-point kernel (sm_90a).
 //
 // One CTA of W warps owns one QP for the whole solve: Mehrotra predictor-corrector iterations around a
 // square-root Riccati factorisation / substitution, with residuals, step length, centring and the

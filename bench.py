@@ -36,7 +36,7 @@ UNIT = "QP/s"
 
 
 # BASELINE.json configs: (metric suffix, default batch per GPU, description).  c2 is the configuration the metric is quoted on and
-# the default; the others are the parity-test shapes, measurable with --config for the per-shape lines of DESIGN.md section 5b.
+# the default; the others are the parity-test shapes, measurable with --config.
 CONFIGS = {
     "c2": ("chain-mass N=40", 4096, "chain-of-masses OCP-QP nx=21 nu=3 N=40 (after x0 elimination), nbu=3 hard + 4 one-sided soft state bounds (ns=4)"),
     "c1": ("mass-spring N=15", 16384, "mass_spring_example OCP-QP nx=8 nu=3 N=15 (after x0 elimination), input and state boxes"),
@@ -128,8 +128,12 @@ class ClockSampler:
         self.thread.join(timeout=1.0)
         sm = [m for m, _ in self.samples]
         reasons = sorted({name for _, r in self.samples for name, bit in self.REASONS if r & bit})
+        try:
+            power_limit_w = self.nv.nvmlDeviceGetEnforcedPowerLimit(self.h) / 1000.0
+        except Exception:  # noqa: BLE001
+            power_limit_w = None
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": self.smmax, "reasons": reasons, "samples": len(sm),
-                "source": "NVML, 10 ms period, timed region only"}
+                "power_limit_w": power_limit_w, "source": "NVML, 10 ms period, timed region only"}
 
 
 def cpu_reference(batch_obj, opts, nqp: int, threads: int = 0):
@@ -157,6 +161,29 @@ def cpu_reference(batch_obj, opts, nqp: int, threads: int = 0):
             "value_incl_struct_packing": nqp / wall}, sol, info
 
 
+DUMP_BYTES = 60 * 10**6      # stays under 64 MB with the .npy headers
+
+
+def dump_outputs(out_dir: str, d_sol, d_info):
+    """What a caller of the device-resident solve receives for the batch of the last timed step: the solution records
+    (sol.npy, one row per QP; a fixed, seeded sample of rows when the whole batch exceeds 60 MB, their indices in
+    sol_rows.npy) and every per-QP field of the info records (info_<field>.npy), all as float64."""
+    import torch
+    from acados_b200.binding import INFO_DTYPE
+    os.makedirs(out_dir, exist_ok=True)
+    nb, stride = d_sol.shape
+    info = np.frombuffer(d_info.cpu().numpy().tobytes(), dtype=INFO_DTYPE)
+    fields = [f for f in INFO_DTYPE.names if f != "reserved"]
+    info_bytes = sum(8 * nb * int(np.prod(INFO_DTYPE[f].shape or (1,))) for f in fields)
+    rows = max(1, min(nb, (DUMP_BYTES - info_bytes - 8 * nb) // (8 * stride)))
+    idx = np.arange(nb) if rows == nb else np.sort(np.random.default_rng(0).choice(nb, rows, replace=False))
+    sol = d_sol[torch.from_numpy(idx).to(d_sol.device)].cpu().numpy()
+    np.save(os.path.join(out_dir, "sol.npy"), np.ascontiguousarray(sol, dtype=np.float64))
+    np.save(os.path.join(out_dir, "sol_rows.npy"), idx.astype(np.float64))
+    for f in fields:
+        np.save(os.path.join(out_dir, f"info_{f}.npy"), np.ascontiguousarray(info[f], dtype=np.float64))
+
+
 def main():
     # the contract is ONE line on stdout: keep the real stdout aside and send everything else that writes to file descriptor 1
     # (NCCL prints its version banner there when a communicator is created) to stderr
@@ -175,12 +202,16 @@ def main():
     ap.add_argument("--fast", type=int, default=1, help="0: keep the throughput kernel off (generic one-warp-per-QP kernel only)")
     ap.add_argument("--target-batch", type=int, default=0, help="QPs per GPU of the extra target-point measurement (default: 8192 when the job has 8 ranks)")
     ap.add_argument("--e2e-pipe", type=int, default=1, help="chunks per host call in the e2e leg (0: the solver's default of 8, best for one blocking call; "
-                    "1: the whole batch per call, best when two solver objects alternate -- measured 107 k vs 88 k QP/s)")
+                    "1: the whole batch per call, best when two solver objects alternate)")
     ap.add_argument("--no-scatter", action="store_true", help="N > 1: skip the scatter / solve / gather leg over NCCL")
     ap.add_argument("--no-plugin", action="store_true", help="skip the end-to-end leg through the plugin's batched entry")
     ap.add_argument("--no-tight", action="store_true", help="skip the second parity pass (all tolerances 1e-12)")
     ap.add_argument("--config", default="c2", choices=sorted(CONFIGS), help="BASELINE.json configuration (default c2: the one the metric is quoted on)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the last device-resident step computed as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     global _CONFIG, METRIC
     _CONFIG = args.config
     if args.batch <= 0:
@@ -197,7 +228,7 @@ def main():
     config = {"workload": f"{CONFIGS[_CONFIG][2]}, batch={args.batch} per GPU, every QP its own matrices", "name": _CONFIG,
               "batch_per_gpu": args.batch, "global_batch": args.batch * max(world, 1), "parallelism": f"batch-sharded x{max(world,1)}",
               "solver_opts": "acados defaults: BALANCE mode, iter_max=50, tol 1e-6/1e-8/1e-8/1e-8, mu0=1, cold start",
-              "l2": "inputs (hundreds of MB to GB per batch) exceed the 126 MB L2; no explicit flush"}
+              "l2": "inputs (hundreds of MB to GB per batch) exceed the 50 MB L2; no explicit flush"}
 
     # ------------------------------------------------------------------------------------------------
     if args.impl == "reference":
@@ -275,6 +306,8 @@ def main():
     launches_per_step = solver.last_launch_count
     clocks = sampler.stop()
     dev_ms = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_sol, d_info)
     # per-launch duration of the solve kernel (events recorded around each launch by the solver itself)
     solver.solve_device(nb, d_qp.data_ptr(), d_sol.data_ptr(), d_info.data_ptr(), opts, sync=True)
     solve_ms = solver.last_kernel_ms                 # all kernels of one solve (repack, throughput kernel, generic kernel over hand-backs)
@@ -427,50 +460,28 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        fp64 = {}
-        try:
-            fp64 = json.load(open(os.path.join(ROOT, "profiles", "r02_fp64_peak.json")))
-        except Exception:
-            pass
-        fp64_peak = float(fp64.get("dfma_tflops", 33.9))
+        # H100 SXM data sheet: 3.35 TB/s of HBM3, 34 TFLOP/s FP64 on the CUDA cores (67 with FP64 tensor cores), for a card
+        # allowed 700 W; a power-limited card reaches less
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+        fp64_peak = 34.0
         ab = algorithmic_bytes_per_qp(b)
         achieved = ab["B_min"] * nb / (kernel_ms * 1e-3) / 1e9
         stream_gbs = ab["B_stream_iter"] * iters_mean * nb / (kernel_ms * 1e-3) / 1e9
         tflops = flops_per_qp(b, iters_mean) * nb / (kernel_ms * 1e-3) / 1e12
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tp):
-            try:
-                traffic = json.load(open(tp)).get("dram_bytes_per_launch")
-            except Exception:
-                traffic = None
-        ncu = {}
-        tp = os.path.join(ROOT, "profiles", "r02_ncu_headline.json")
-        if os.path.exists(tp):
-            try:
-                ncu = json.load(open(tp))
-            except Exception:
-                ncu = {}
-        if traffic is None:
-            traffic = ncu.get("dram_bytes_per_launch")
-        if _CONFIG != "c2" or nb != 4096:       # the committed ncu capture is of the headline configuration
-            traffic, ncu = None, {}
         # SURVEY 8(d): the path is bounded by the FP64 pipe or by HBM; frac = the larger of the two fractions.  HBM term on
         # ALGORITHMIC bytes (B_min: every record read once, the solution written once), FP64 term on algorithmic flops against
-        # the DFMA rate measured on this GPU type (scripts/ubench_fp64.cu -> profiles/r02_ubench_fp64.txt).
+        # the data-sheet FP64 rate of the CUDA cores.
         frac_hbm, frac_fp64 = achieved / hbm_peak, tflops / fp64_peak
         roofline = {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": max(frac_hbm, frac_fp64),
                     "frac_hbm_algorithmic": frac_hbm, "frac_fp64_algorithmic": frac_fp64, "frac_is": "fp64" if frac_fp64 > frac_hbm else "hbm",
-                    "traffic": traffic, "kernel": ("cuipm_fast_kernel (ring loop + first launch of the iteration-sliced scheduling)" if launches_per_step > 3 else "cuipm_fast_kernel") if args.fast and launches_per_step > 1 else "cuipm_solve_kernel",
+                    "kernel": ("cuipm_fast_kernel (ring loop + first launch of the iteration-sliced scheduling)" if launches_per_step > 3 else "cuipm_fast_kernel") if args.fast and launches_per_step > 1 else "cuipm_solve_kernel",
                     "kernel_ms": kernel_ms, "solve_ms_all_kernels": solve_ms,
-                    "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (of fallback)",
+                    "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s",
                     "algorithmic_bytes_per_qp": ab["B_min"], "mean_ipm_iterations": iters_mean,
                     "stream_model": {"bytes_per_qp": ab["B_stream_iter"] * iters_mean, "achieved_gbs": stream_gbs, "frac": stream_gbs / hbm_peak},
                     "fp64": {"achieved_tflops": tflops, "peak_tflops": fp64_peak,
-                             "peak_source": "measured DFMA rate, profiles/r02_ubench_fp64.txt" if fp64 else "33.9 TFLOP/s (measured earlier on a B200 of this pool)",
-                             "frac": frac_fp64, "ncu_pipe_fp64_cycles_active_pct": ncu.get("sm__pipe_fp64_cycles_active_pct")},
-                    "ncu": ncu or None}
+                             "peak_source": "H100 SXM data sheet, FP64 without tensor cores",
+                             "frac": frac_fp64}}
         cpu, parity = None, None
         if not args.no_cpu:
             try:
@@ -510,13 +521,13 @@ def main():
                 cpu = {"value": None, "unit": UNIT, "cores": 0, "kind": "unavailable", "sample": str(e)}
         line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": steps, "warmup": warmup,
                 "ms_per_step": dev_ms / steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                "dtype": "f64", "data": "synthetic", "config": config, "clocks": clocks,
+                "dtype": "f64", "data": "synthetic", "config": config, "device": torch.cuda.get_device_name(local_rank), "clocks": clocks,
                 "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(b.qp.nbytes) * world,
                         "d2h_bytes_per_step": int(h_sol.numel() * 8 + h_info.numel()) * world, "ms_per_step": e2e_ms / steps,
                         "lanes": 2, "chunks_per_call": args.e2e_pipe or 8,
                         "note": "two solver objects alternate (cuipm_solve_host_async / cuipm_wait): the copies of step i+1 overlap the solve "
                         "of step i; every call moves its whole batch in one piece (tuning key pipe=1) so that the solve runs with the "
-                        "iteration-sliced scheduling (8 chunks per call -- the default, best for a single blocking call -- give 88 k QP/s here)"},
+                        "iteration-sliced scheduling (8 chunks per call are the default, best for a single blocking call)"},
                 "e2e_plugin": plugin, "scatter_gather": sg, "target_point": target,
                 "gpu_launches": steps * launches_per_step,
                 "roofline": roofline, "cpu_baseline": cpu, "parity": parity,

@@ -1,5 +1,5 @@
 /*
- * cuipm.h -- C ABI of the B200-native batched OCP-QP interior-point solver.
+ * cuipm.h -- C ABI of the H100-native batched OCP-QP interior-point solver.
  *
  * This is the drop-in boundary for acados' `qp_solver` plugin slot: everything the reference's
  * `ocp_qp_hpipm()` (acados/ocp_qp/ocp_qp_hpipm.c:314-405) obtains from HPIPM's

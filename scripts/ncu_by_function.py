@@ -13,7 +13,7 @@ if "--cubin" in sys.argv:
 else:
     tmp = tempfile.mkdtemp()
     subprocess.run(["cuobjdump", "-xelf", "all", os.path.join(ROOT, "acados_b200", "csrc", "libcuipm.so")], cwd=tmp, stdout=subprocess.DEVNULL)
-    cubin = os.path.join(tmp, "cuipm_fast.sm_100a.cubin")
+    cubin = os.path.join(tmp, "cuipm_fast.sm_90a.cubin")
 dis = subprocess.run(["nvdisasm", "--print-line-info", cubin], stdout=subprocess.PIPE, text=True).stdout
 core = sys.argv[sys.argv.index("--core") + 1] if "--core" in sys.argv else os.path.join(ROOT, "acados_b200", "csrc", "cuipm_fast_core.h")
 src = open(core).read().split("\n")

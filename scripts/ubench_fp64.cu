@@ -1,6 +1,6 @@
-// ubench_fp64.cu -- FP64 micro-benchmarks on B200 (sm_100a): DFMA and DMMA (mma.sync m8n8k4.f64) issue rates as a
+// ubench_fp64.cu -- FP64 micro-benchmarks on H100 (sm_90a): DFMA and DMMA (mma.sync m8n8k4.f64) issue rates as a
 // function of resident warps per SM and independent chains per thread, dependent-issue latencies of DFMA / rsqrt /
-// shared-memory loads.  Output feeds the roofline denominator of bench.py (profiles/r02_fp64_peak.md).
+// shared-memory loads: the measured rates, to set beside the data-sheet FP64 peak bench.py's roofline divides by.
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

@@ -31,10 +31,11 @@ def cases():
 CASES = dict(cases())
 
 
-def _compare_with_reference(b, o, allow_lq_shift=True):
+def _compare_with_reference(b, o, allow_lq_shift=True, answers=None):
+    """The oracle against the reference on batch b: the live reference, or its stored ``answers`` (sol, info, stat)."""
     from oracle import oracle_binding as ob
     s1, i1, st1 = ob.oracle_solve(b, o, want_stat=True)
-    s2, i2, st2, _ = ob.ref_solve(b, o, want_stat=True, nthreads=1)
+    s2, i2, st2 = answers if answers is not None else ob.ref_solve(b, o, want_stat=True, nthreads=1)[:3]
     assert np.array_equal(i1["iter"], i2["iter"]), (i1["iter"], i2["iter"])
     assert np.array_equal(i1["status"], i2["status"])
     # LQ refactorisation (x_ocp_qp_ipm.c:2299-2330): the switch is triggered by the round-off level of a Cholesky step
@@ -65,23 +66,28 @@ def test_oracle_matches_reference(built, name, lq):
     _compare_with_reference(CASES[name](), default_opts(lq_fact=lq), allow_lq_shift=(lq == 1))
 
 
-@pytest.mark.parametrize("name", ["c1_mass_spring", "c2_chain_mass", "rand_soft", "rand_masked"])
-@pytest.mark.parametrize("tau", [1e-4, 1e-2])
+TAU_MIN_CASES = ["c1_mass_spring", "c2_chain_mass", "rand_soft", "rand_masked"]
+TAU_MIN_VALUES = [1e-4, 1e-2]
+
+
+@pytest.mark.parametrize("name", TAU_MIN_CASES)
+@pytest.mark.parametrize("tau", TAU_MIN_VALUES)
 def test_oracle_matches_reference_with_tau_min(built, name, tau):
     """acados' ``tau_min`` option (ocp_qp_hpipm.c:170-174, 338-342): every entry of qp->m is set to it, the complementarity
     residual becomes lam*t - m and the ratio test switches to the quadratic rule that keeps lam*t >= m_safe*m
-    (x_core_qp_ipm_aux.c:398-440).  Same iteration counts, same solution."""
+    (x_core_qp_ipm_aux.c:398-440).  Same iteration counts, same solution as the reference, whose answers are stored in
+    tests/golden/reference/tau_min.npz (tests/golden/make_reference_answers.py)."""
     from oracle import oracle_binding as ob
-    if not ob.have_ref():
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
     b = CASES[name]()
+    g = np.load(os.path.join(GOLD, "reference", "tau_min.npz"), allow_pickle=False)
+    key = f"{name}_{tau:g}"
+    assert np.array_equal(np.asarray(b.qp[:, :16]), g[key + "_qp_head"]), "generator drifted from the golden inputs"
     o = default_opts(m_relax=tau)
     s1, i1 = ob.oracle_solve(b, o)
-    s2, i2, _ = ob.ref_solve(b, o, nthreads=1)
-    assert np.array_equal(i1["iter"], i2["iter"]), (i1["iter"], i2["iter"])
-    assert np.array_equal(i1["status"], i2["status"])
-    conv = i2["status"] == 0
-    assert np.max(np.abs(b.layout.u_traj(s1) - b.layout.u_traj(s2))[conv], initial=0.0) <= TOL_U
+    assert np.array_equal(i1["iter"], g[key + "_iter"]), (i1["iter"], g[key + "_iter"])
+    assert np.array_equal(i1["status"], g[key + "_status"])
+    conv = g[key + "_status"] == 0
+    assert np.max(np.abs(b.layout.u_traj(s1) - g[key + "_u"])[conv], initial=0.0) <= TOL_U
     # and the option does something: the relaxed problem stops at another point than the unrelaxed one
     s0, _ = ob.oracle_solve(b, default_opts())
     assert np.max(np.abs(s1 - s0)) > 1e-8
@@ -94,14 +100,28 @@ LQ_CASES = {
 }
 
 
+def _stored_lq_answers(name, b):
+    """What the reference returned on LQ case ``name`` (tests/golden/reference/lq_cases.npz): the solution in float32 with its
+    inputs in float64, the statistics table in float32, as (sol, info, stat)."""
+    g = np.load(os.path.join(GOLD, "reference", "lq_cases.npz"), allow_pickle=False)
+    assert np.array_equal(np.asarray(b.qp[:, :16]), g[name + "_qp_head"]), "generator drifted from the golden inputs"
+    sol = g[name + "_sol"].astype(np.float64)
+    u, col = g[name + "_u"], 0
+    for k in range(b.shape.N + 1):
+        nu = b.shape.nu[k]
+        b.layout.view(sol, "ux", k)[:, :nu] = u[:, col:col + nu]
+        col += nu
+    info = {f: g[name + "_" + f] for f in ("iter", "status", "lq_count")}
+    return sol, info, g[name + "_stat"].astype(np.float64)
+
+
 @pytest.mark.parametrize("name", list(LQ_CASES))
 def test_oracle_lq_refactorisation(built, name):
     """Near-singular instances on which the reference switches from Cholesky to its LQ refactorisation
-    (OCP_QP_FACT_LQ_SOLVE_KKT_STEP, x_ocp_qp_kkt.c:1201-1541): same trajectory, same iteration counts."""
-    from oracle import oracle_binding as ob
-    if not ob.have_ref():
-        pytest.skip("oracle/_ref not built (needs /root/reference)")
-    i2 = _compare_with_reference(LQ_CASES[name](), default_opts(lq_fact=1))
+    (OCP_QP_FACT_LQ_SOLVE_KKT_STEP, x_ocp_qp_kkt.c:1201-1541): same trajectory, same iteration counts as the reference's
+    stored answers (tests/golden/make_reference_answers.py)."""
+    b = LQ_CASES[name]()
+    i2 = _compare_with_reference(b, default_opts(lq_fact=1), answers=_stored_lq_answers(name, b))
     assert (i2["lq_count"] > 0).sum() >= 8      # the case does exercise the path
 
 

