@@ -22,7 +22,7 @@ struct StageDesc
     int pad_;
     unsigned q_BAt, q_RSQ, q_DCt, q_b, q_rq, q_d, q_dmask, q_Z, q_z;
     VOff sol, step, itref;
-    ROff res, ires;
+    ROff res, ires;                       // residual sets 0 and 1; the throughput kernel keeps the affine step (dux, dpi, masked dlam) in ires.g, .b, .d
     unsigned w_rmb, w_L, w_Linv, w_lrow, w_Pb, w_Zsi;
     unsigned q_stage, q_stage_bytes;      // this stage's sub-record inside the QP record (16-byte multiple)
     unsigned w_fac, w_fac_bytes;          // factor part of the work record (L, Linv, lrow, Pb, Zs_inv)

@@ -36,6 +36,12 @@
 
 #include "cuipm_device.h"
 
+// bytes brought into shared memory by one bulk or 16-byte asynchronous copy: a host build can count them (the staged bytes per
+// QP-iteration are what the sweeps of this kernel cost on the H100, tests/test_fast_staged_bytes.py)
+#ifndef FK_COUNT_STAGED
+#define FK_COUNT_STAGED(bytes) do {} while (0)
+#endif
+
 #ifndef FK_PROF_T0
 #define FK_PROF_T0() do {} while (0)
 #define FK_PROF_ADD(slot) do {} while (0)
@@ -87,11 +93,31 @@ namespace fastk {
 
 FK_DEV int evn(int n) { return (n + 1) & ~1; }
 
+// a product rounded before it is used: never contracted into an FMA with the sum it enters (the host build of the emulation
+// has no FMA to contract into)
+FK_DEV double mul_rn(double a, double b)
+{
+#ifdef __CUDA_ARCH__
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+
 // per-QP scalars of the IPM loop
 struct QpState
 {
     double mu, obj, gap, alpha, res_m_tau;
     double res_max[4];
+};
+
+// the residual of the linear system of the iteration just run: inf-norms of its stationarity rows for the affine and the final
+// step (from the residual sweep that applies the step), the tests on its other rows (from the forward sweeps), res_max[0] of
+// the iterate the steps were computed at
+struct LinNrm
+{
+    double aff_g, fin_g, res0_g;
+    bool aff_bdm_large, fin_bdm_small;
 };
 
 template <int NX, int NU, int G>
@@ -271,7 +297,10 @@ struct Ker
     {
         // lane 0 of every group issues the copy of its QP (the compiler serialises the 32/G different operand sets)
         if (li == 0)
+        {
             fk_bulk(smem0 + (size_t) gq * A.gstride + soff, (REC == 0 ? qk : (REC == 1 ? sol : (REC == 2 ? wk : qp))) + off, (unsigned) nd * 8u, bars + BAR);
+            FK_COUNT_STAGED((unsigned) nd * 8u);
+        }
         (void) pf;
         if (BAR == 0) tx0 += (unsigned) (QPW * nd) * 8u;
         else tx1 += (unsigned) (QPW * nd) * 8u;
@@ -285,7 +314,11 @@ struct Ker
     {
         const double *src = (REC == 0 ? qk : (REC == 1 ? sol : (REC == 2 ? wk : qp))) + off;
 FK_VLOOP
-        for (int e = 2 * li; e < nd; e += 2 * G) fk_cp16(dst + e, src + e);
+        for (int e = 2 * li; e < nd; e += 2 * G)
+        {
+            fk_cp16(dst + e, src + e);
+            FK_COUNT_STAGED(16u);
+        }
     }
     // all lanes are done with the buffers the next copies overwrite
     FK_DEV void stage_begin() { fk_fence_async(); fk_sync(); }
@@ -424,10 +457,60 @@ FK_PRAGMA(unroll FK_U_DOT)
     {
         double a_mu, a_obj, a_gap, m0, m1, m2, m3, m4;
         int f0, f1, f2, f3, f4;
+        // stationarity rows of the residual of the linear system: inf-norms for the affine (a) and the final (f) step, and
+        // dpi of the stage before for the rows of this lane (entry m: row li + G m)
+        double ma, mf, pa[RPM > 0 ? RPM : 1], pf[RPM > 0 ? RPM : 1];
+        int fa, ff;
     };
 
+    // stationarity rows of the residual of the linear system of one step (dux, dpi_k, dlam: du, dp, dl; dl is masked unless mask_dl;
+    // dpi_{k-1}: pm) -> inf-norm mx / NaN flag fl:  ((H dux + rhs_g) - dpi_{k-1} + A dpi_k) + bound multipliers, slack rows
+    // Z ds + rhs_g - multipliers; a masked multiplier step is rounded before it is summed (OCP_QP_RES_COMPUTE_LIN).  ML, MA:
+    // Hessian and dynamics block; rg: rhs_g (residual set 0 of the iterate the step was computed at).
     template <int KIND>
-    FK_DEV void res_stage(int k, int update, double alpha_u, ResAcc &R)
+    FK_DEV void lin_rows(const double *du, const double *dp, const double *dl, bool mask_dl, const double *msk, const double *rg,
+                         const double *qZ, const int *idxb, const int *rev, const int *inv, int nb, int ns, const double (&pm)[RPM > 0 ? RPM : 1],
+                         double &mx, int &fl) const
+    {
+        constexpr int nx = KD<KIND>::nx, nu = KD<KIND>::nu, n = nx + nu, nx1 = KD<KIND>::nx1;
+        constexpr int RP = (n + G - 1) / G;
+        double hx[RPM > 0 ? RPM : 1], ap[RPM > 0 ? RPM : 1];
+        rows_dot<n, n>(ML, LDK, du, hx);
+        if (nx1 > 0) rows_dot<n, nx1>(MA, LDK, dp, ap);
+#pragma unroll
+        for (int m = 0; m < RP; m++)
+        {
+            const int i = li + G * m;
+            if (i < n)
+            {
+                double r = hx[m] + rg[i];
+                if (nx > 0 && i >= nu) r -= pm[m];
+                if (nx1 > 0) r += ap[m];
+                // the bound on row i (at most one: the throughput kernel takes no repeated index in idxb)
+                for (int b = 0; b < nb; b++)
+                    if (idxb[b] == i)
+                        r += (mask_dl ? mul_rn(dl[nb + b], msk[nb + b]) : dl[nb + b]) - (mask_dl ? mul_rn(dl[b], msk[b]) : dl[b]);
+                const double a = fabs(r);
+                mx = fmax(mx, a);
+                fl |= (a != a);
+            }
+        }
+FK_VLOOP
+        for (int j = li; j < 2 * ns; j += G)
+        {
+            double r = qZ[j] * du[n + j] + rg[n + j] - (mask_dl ? mul_rn(dl[2 * nb + j], msk[2 * nb + j]) : dl[2 * nb + j]);
+            const int jj = j < ns ? j : j - ns, offl = j < ns ? 0 : nb;
+            FK_FOR_SLACK(i, jj) r -= mask_dl ? mul_rn(dl[offl + i], msk[offl + i]) : dl[offl + i];
+            const double a = fabs(r);
+            mx = fmax(mx, a);
+            fl |= (a != a);
+        }
+    }
+
+    // lin_a / lin_f: also the stationarity rows of the residual of the linear system for the affine step (kept by the forward
+    // sweep in ires) / for the step applied (update only)
+    template <int KIND>
+    FK_DEV void res_stage(int k, int update, bool lin_a, bool lin_f, double alpha_u, ResAcc &R)
     {
         constexpr int nx = KD<KIND>::nx, nu = KD<KIND>::nu, n = nx + nu, nx1 = KD<KIND>::nx1;
         constexpr int RP = (n + G - 1) / G, CP = (nx1 + G - 1) / G;
@@ -441,12 +524,16 @@ FK_PRAGMA(unroll FK_U_DOT)
         const int qvN = (int) ((sd.q_stage + sd.q_stage_bytes / 8u) - sd.q_b);
         double *SOL = V, *STP = SOL + (A.nve + NXe + 2 * A.nce), *SOLN = STP + (A.nve + NXe + 2 * A.nce), *STPN = SOLN + NMe;
         double *QV = STPN + NMe, *tmp0 = QV + (NXe + NMe + 2 * A.nce + 2 * A.ns2e), *tmp1 = tmp0 + A.nbe, *g_ = tmp1 + A.nbe, *pim = g_ + A.nve;
-        double *x1 = pim + NXe;
+        double *x1 = pim + NXe, *AF = x1 + NXe;
         const int pf = (KIND == 1 && k + 1 < A.N) ? 1 : 0;
         stage_begin();
         vcopy<1>(SOL, (size_t) v.kk * A.ss + sd.sol.ux, solN);
         if (update) vcopy<2>(STP, (size_t) v.kk * A.ws + sd.step.ux, stpN);
         vcopy<0>(QV, (size_t) A.kq[KIND] + (size_t) v.kk * A.kqs + A.kV[KIND], evn(qvN));
+        // rhs_g of the linear system = the residual set 0 this stage overwrites: staged in g_, every row is read (lin_rows) by
+        // the lane that later writes it, before it does
+        if (lin_a || lin_f) vcopy<2>(g_, (size_t) v.kk * A.ws + sd.res.g, evn(n + 2 * ns));
+        if (lin_a) vcopy<2>(AF, (size_t) v.kk * A.ws + sd.ires.g, (int) (sd.ires.d - sd.ires.g) + evn(nc));
         if (nx1 > 0)
         {
             const StageDesc &s1 = sdr(k + 1);
@@ -516,6 +603,8 @@ FK_VLOOP
         for (int i = li; i < nb; i += G) tmp0[i] = lam[nb + i] - lam[i];
         wait_mat();
         fk_sync();
+        if (lin_a) lin_rows<KIND>(AF, AF + (sd.ires.b - sd.ires.g), AF + (sd.ires.d - sd.ires.g), false, msk, g_, qZ, idxb, rev, inv, nb, ns, R.pa, R.ma, R.fa);
+        if (lin_f) lin_rows<KIND>(du, dp, dl, true, msk, g_, qZ, idxb, rev, inv, nb, ns, R.pf, R.mf, R.ff);
         // ---- rows of res_g (lane = row), res_b (lane = column)
         {
             double hx[RPM > 0 ? RPM : 1], ap[RPM > 0 ? RPM : 1];
@@ -642,19 +731,42 @@ FK_VLOOP
         }
 FK_VLOOP
         for (int j = li; j < nx1; j += G) pim[j] = pi[j];      // pi_k is "pi_{k-1}" of the next stage
+        if (nx1 > 0 && (lin_a || lin_f))
+        {
+            // the entries of dpi_k the rows of this lane take in the next stage (row i: i - nu of that stage)
+            const int nun = k + 1 < A.N ? NU : 0;
+            const double *dpa = AF + (sd.ires.b - sd.ires.g);
+#pragma unroll
+            for (int m = 0; m < RPM; m++)
+            {
+                const int j = li + G * m - nun;
+                const bool in = j >= 0 && j < nx1;
+                R.pa[m] = in && lin_a ? dpa[j] : 0.0;
+                R.pf[m] = in && lin_f ? dp[j] : 0.0;
+            }
+        }
     }
 
-    FK_DEV void res_pass(int update, double alpha_u, QpState &Q)
+    // update: move along the step first; then also the stationarity norms of the residual of the linear system of the iteration
+    // that computed the step, into L.aff_g / L.fin_g (lin_check tests them)
+    FK_DEV void res_pass(int update, double alpha_u, QpState &Q, LinNrm &L)
     {
         fk_fence_async_global();        // the records this sweep reads with bulk copies were written with plain stores by the sweeps before
 
+        const bool lin_a = update && A.o.lq_fact == 1, lin_f = update && A.o.pred_corr == 1 && A.o.itref_corr_max > 0;
         ResAcc R;
         R.a_mu = R.a_obj = R.a_gap = R.m0 = R.m1 = R.m2 = R.m3 = R.m4 = 0.0;
         R.f0 = R.f1 = R.f2 = R.f3 = R.f4 = 0;
+        R.ma = R.mf = 0.0;
+        R.fa = R.ff = 0;
+#pragma unroll
+        for (int m = 0; m < (RPM > 0 ? RPM : 1); m++) R.pa[m] = R.pf[m] = 0.0;
         if (update && alpha_u < 1.0) alpha_u = alpha_u * ((1.0 - alpha_u) * 0.99 + alpha_u * 0.9999999);
-        res_stage<0>(0, update, alpha_u, R);
-        for (int k = 1; k < A.N; k++) res_stage<1>(k, update, alpha_u, R);
-        res_stage<2>(A.N, update, alpha_u, R);
+        res_stage<0>(0, update, lin_a, lin_f, alpha_u, R);
+        for (int k = 1; k < A.N; k++) res_stage<1>(k, update, lin_a, lin_f, alpha_u, R);
+        res_stage<2>(A.N, update, lin_a, lin_f, alpha_u, R);
+        if (lin_a) L.aff_g = gmax_nan(R.ma, R.fa);
+        if (lin_f) L.fin_g = gmax_nan(R.mf, R.ff);
         Q.res_max[0] = gmax_nan(R.m0, R.f0);
         Q.res_max[1] = gmax_nan(R.m1, R.f1);
         Q.res_max[2] = gmax_nan(R.m2, R.f2);
@@ -1375,15 +1487,18 @@ FK_VLOOP
     // ---------------------------------------------------------------------------------------------
     // one stage of the forward sweep (x_ocp_qp_kkt.c:968-1006 / 1682-1722) + step of the constraint variables
     // (:1176-1193, EXPAND_SLACKS :524-598, COMPUTE_LAM_T_QP x_core_qp_ipm_aux.c:164-189) + the ratio test
-    // (COMPUTE_ALPHA_QP :375-398) + the residual of the linear system (OCP_QP_RES_COMPUTE_LIN) -> residual set 1.
+    // (COMPUTE_ALPHA_QP :375-398) + the norms of the b, d and m rows of the residual of the linear system
+    // (OCP_QP_RES_COMPUTE_LIN).  Its stationarity rows need the Hessian: the residual sweep that applies the step computes
+    // them (res_stage), so this sweep streams the factor only.  The affine step (after_fact) is overwritten by the
+    // corrector before that sweep: with do_lin its dux, dpi and masked dlam are kept in the residual set 1 area of the work
+    // record (ires.g / .b / .d), which this kernel uses for nothing else.
     // after_fact: start from -lrow, pi = P x + p with p from lrow; else: start from the backward quantities stored in
     // the step, pi = p_backward + P x.
-    // ML first holds the Hessian (for the residual of the linear system), then the factor of the next stage.
     // ---------------------------------------------------------------------------------------------
     struct FwdAcc
     {
-        double alpha, m0, m1, m2, m3;
-        int f0, f1, f2, f3;
+        double alpha, m1, m2, m3;
+        int f1, f2, f3;
     };
 
     template <int KIND>
@@ -1391,30 +1506,29 @@ FK_VLOOP
     {
         constexpr int nx = KD<KIND>::nx, nu = KD<KIND>::nu, n = nx + nu, nx1 = KD<KIND>::nx1;
         constexpr int nsolve = nu;
-        constexpr int RP = (n + G - 1) / G, CP = (nx1 + G - 1) / G;
+        constexpr int CP = (nx1 + G - 1) / G;
         FK_PROF_T2();
         const StageDesc &sd = sdk<KIND>();
         const View v = view<KIND>(k);
         const int nb = sd.nb, ns = sd.ns, nc = sd.nc;
         const int *idxb = IDX + 4 * (A.nmaps == 3 ? KIND : k) * A.nbe, *rev = idxb + nb, *inv = rev + nb;
         const int nu1 = (nx1 > 0 && k + 1 < A.N) ? NU : 0, n1 = nx1 + nu1, n1e = (n1 + 1) & ~1;
-        const int resN = (int) (sd.res.m - sd.res.g) + evn(nc), ltN = (int) (sd.sol.t - sd.sol.lam) + evn(nc);
-        const int fvN = (int) (sd.w_Zsi - sd.w_Linv) + evn(2 * ns), qmN = (int) (sd.q_Z - sd.q_dmask) + evn(2 * ns);
+        const int resN = (int) (sd.res.m - sd.res.b) + evn(nc), ltN = (int) (sd.sol.t - sd.sol.lam) + evn(nc);
+        const int fvN = (int) (sd.w_Zsi - sd.w_Linv) + evn(2 * ns);
         double *RES = V, *LT = RES + (A.nve + NXe + 2 * A.nce), *FV = LT + 2 * A.nce, *SUX = FV + (2 * NMe + NXe + A.ns2e), *P1 = SUX + A.nve;
-        double *QM = P1 + NMe, *vv = QM + (A.nce + A.ns2e), *x1 = vv + A.nve, *tg = x1 + NXe, *pik = tg + A.nve, *pim = pik + NXe;
-        double *dt = pim + NXe, *dlm = dt + A.nce, *dsv = dlm + A.nce, *tmp0 = dsv + A.ns2e;
-        double *tmp = tg, *g_ = tg;                 // tmp (Lxx' x) is dead when g_ (residual rows) is written
-        const bool so = act && stw;
+        double *QM = P1 + NMe, *vv = QM + (A.nce + A.ns2e), *x1 = vv + A.nve, *tmp = x1 + NXe;
+        double *dt = tmp + A.nve, *tis = dt + A.nce, *dsv = tis + A.nce;
+        const bool so = act && stw, sa = so && after_fact && do_lin;      // sa: keep the affine step for the residual sweep
         View v1 = v;
         const StageDesc *s1p = &sd;
         if (nx1 > 0) { s1p = &sdr(k + 1); v1 = viewr(k + 1); }
         const int pf = (KIND == 1 && k + 2 < A.N) ? 1 : 0;
         stage_begin();
-        vcopy<2>(RES, (size_t) v.kk * A.ws + sd.res.g, resN);
+        vcopy<2>(RES, (size_t) v.kk * A.ws + sd.res.b, resN);
         vcopy<1>(LT, (size_t) v.kk * A.ss + sd.sol.lam, ltN);
         vcopy<2>(FV, (size_t) v.kk * A.ws + sd.w_Linv, fvN);
         vcopy<2>(SUX, (size_t) v.kk * A.ws + sd.step.ux, evn(n + 2 * ns));
-        vcopy<0>(QM, (size_t) A.kq[KIND] + (size_t) v.kk * A.kqs + A.kV[KIND] + (sd.q_dmask - sd.q_b), qmN);
+        vcopy<0>(QM, (size_t) A.kq[KIND] + (size_t) v.kk * A.kqs + A.kV[KIND] + (sd.q_dmask - sd.q_b), evn(nc));
         if (nx1 > 0)
         {
             // p part (gradient vector of stage k+1) / backward value of x_{k+1}
@@ -1422,14 +1536,13 @@ FK_VLOOP
             bulk<0, 1>(voff(MA), (size_t) A.kq[KIND] + (size_t) v.kk * A.kqs, evn(LDK * nx1), pf);
         }
         if (nsolve > 0) bulk<2, 1>(voff(LU), (size_t) v.kk * A.ws + sd.w_L, evn(n * nsolve), pf);
-        if (do_lin) bulk<0, 1>(voff(ML), (size_t) A.kq[KIND] + (size_t) v.kk * A.kqs + A.kH[KIND], evn(LDK * n), pf);
-        else if (nx1 > 0) bulk<2, 1>(voff(ML), (size_t) v1.kk * A.ws + s1p->w_Lxx, evn((nx1 | 1) * nx1), pf);
+        if (nx1 > 0) bulk<2, 1>(voff(ML), (size_t) v1.kk * A.ws + s1p->w_Lxx, evn((nx1 | 1) * nx1), pf);
         stage_arm();
         wait_vec();
-        const double *gv = RES, *bs = RES + (sd.res.b - sd.res.g), *rds = RES + (sd.res.d - sd.res.g), *rms = RES + (sd.res.m - sd.res.g);
+        const double *bs = RES, *rds = RES + (sd.res.d - sd.res.b), *rms = RES + (sd.res.m - sd.res.b);
         const double *lam = LT, *ts = LT + (sd.sol.t - sd.sol.lam);
         const double *Lis = FV, *lrow_ = FV + (sd.w_lrow - sd.w_Linv), *Zi = FV + (sd.w_Zsi - sd.w_Linv);
-        const double *mks = QM, *qZ = QM + (sd.q_Z - sd.q_dmask);
+        const double *mks = QM;
         {
             const double *src = after_fact ? lrow_ : SUX;
 FK_VLOOP
@@ -1469,31 +1582,20 @@ FK_VLOOP
             fk_sync();
         }
         {
-            double *o_ = v.w + sd.step.ux;
+            double *o_ = v.w + sd.step.ux, *oa = v.w + sd.ires.g;
 FK_VLOOP
             for (int i = li; i < n; i += G)
-                if (so) o_[i] = vv[i];
-        }
-        FK_PROF_ADD2(17);      /* u */
-        // ---- H v (for the residual of the linear system) while ML holds the Hessian, then ML <- L_{k+1}
-        double hx[RPM > 0 ? RPM : 1];
-        if (do_lin)
-        {
-            rows_dot<n, n>(ML, LDK, vv, hx);
-            if (nx1 > 0)
             {
-                stage_begin();
-                bulk<2, 1>(voff(ML), (size_t) v1.kk * A.ws + s1p->w_Lxx, evn((nx1 | 1) * nx1), pf);
-                stage_arm_mat();
+                if (so) o_[i] = vv[i];
+                if (sa) oa[i] = vv[i];
             }
         }
-        FK_PROF_ADD2(18);      /* H v */
+        FK_PROF_ADD2(17);      /* u */
         // ---- x+ = A' v + b
         if (nx1 > 0)
         {
             double av[RPM > 0 ? RPM : 1];
             cols_dot<n, nx1>(MA, LDK, vv, av);
-            double *ob = v.w + sd.ires.b;
 #pragma unroll
             for (int m = 0; m < CP; m++)
             {
@@ -1506,7 +1608,6 @@ FK_VLOOP
                     if (do_lin)
                     {
                         const double r = bv - xj + acc;
-                        if (so) ob[j] = r;
                         const double a = fabs(r);
                         F.m1 = fmax(F.m1, a);
                         F.f1 |= (a != a);
@@ -1517,8 +1618,6 @@ FK_VLOOP
         FK_PROF_ADD2(19);      /* x+ */
         // ---- constraint part of the step at this stage
         {
-            double *tis = dlm;                   // 1 / t; shares the array of the masked multiplier steps: entry i is read, then
-                                                 // overwritten, by the same lane in the loop over the constraints below
             recip_vec(ts, tis, nc);
 FK_VLOOP
             for (int i = li; i < nb; i += G)
@@ -1553,13 +1652,16 @@ FK_VLOOP
                     const int up = i >= nb, ii = up ? i - nb : i;
                     if (rev[ii] >= 0) dt[i] += dsv[(up ? ns : 0) + rev[ii]];
                 }
-                double *o_ = v.w + sd.step.ux + n;
+                double *o_ = v.w + sd.step.ux + n, *oa = v.w + sd.ires.g + n;
 FK_VLOOP
                 for (int j = li; j < 2 * ns; j += G)
+                {
                     if (so) o_[j] = dsv[j];
+                    if (sa) oa[j] = dsv[j];
+                }
             }
             fk_sync();
-            double *odl = v.w + sd.step.lam, *odt = v.w + sd.step.t, *ld_ = v.w + sd.ires.d, *lm_ = v.w + sd.ires.m;
+            double *odl = v.w + sd.step.lam, *odt = v.w + sd.step.t, *oa = v.w + sd.ires.d;
 FK_VLOOP
             for (int i = li; i < nc; i += G)
             {
@@ -1571,7 +1673,7 @@ FK_VLOOP
                 dl *= mk;
                 dti *= mk;
                 if (so) { odl[i] = dl; odt[i] = dti; }
-                dlm[i] = dl * mk;     // masked step multipliers (tmp_lam_mask of the linear residual)
+                if (sa) oa[i] = dl * mk;       // masked step multipliers (tmp_lam_mask of the linear residual)
                 // ratio test (min over constraints, see COMPUTE_ALPHA_QP)
                 if (l + dl < 0.0) F.alpha = fmin(F.alpha, -l / dl);
                 if (tt + dti < 0.0) F.alpha = fmin(F.alpha, -tt / dti);
@@ -1580,13 +1682,11 @@ FK_VLOOP
                     // res_d = rhs_d + dt -/+ (v[idxb] | C'v) [- ds] = rhs_d + dt - dtr ;  res_m = rhs_m + lam dt + dlam t
                     double r = (dti + rdi) - dtr;
                     r *= mk;
-                    if (so) ld_[i] = r;
                     double a = fabs(r);
                     F.m2 = fmax(F.m2, a);
                     F.f2 |= (a != a);
                     double mm = rmi + l * dti + dl * tt;
                     mm *= mk;
-                    if (so) lm_[i] = mm;
                     a = fabs(mm);
                     F.m3 = fmax(F.m3, a);
                     F.f3 |= (a != a);
@@ -1597,9 +1697,8 @@ FK_VLOOP
         // ---- pi = P x+ + p with the factor of the next stage
         if (nx1 > 0)
         {
-            if (do_lin) wait_mat();
             fk_sync();
-            const double *Lx = ML;                                           // Lxx of stage k+1, odd leading dimension, zero above the diagonal
+            const double *Lx = ML;                                          // Lxx of stage k+1, odd leading dimension, zero above the diagonal
             constexpr int ldx = nx1 | 1;
             double tt_[RPM > 0 ? RPM : 1];
             cols_dot<nx1, nx1>(Lx, ldx, x1, tt_);
@@ -1610,7 +1709,7 @@ FK_VLOOP
                 if (j < nx1) tmp[j] = after_fact ? tt_[m] + P1[nu1 + j] : tt_[m];
             }
             fk_sync();
-            double *pi = v.w + sd.step.pi;
+            double *pi = v.w + sd.step.pi, *oa = v.w + sd.ires.b;
             rows_dot<nx1, nx1>(Lx, ldx, tmp, tt_);
 #pragma unroll
             for (int m = 0; m < CP; m++)
@@ -1620,85 +1719,33 @@ FK_VLOOP
                 {
                     const double pv = after_fact ? tt_[m] : tt_[m] + P1[nu1 + i];
                     if (so) pi[i] = pv;
-                    pik[i] = pv;
+                    if (sa) oa[i] = pv;
                 }
             }
         }
         fk_sync();
         FK_PROF_ADD2(21);      /* pi */
-        if (do_lin)
-        {
-            // ---- res_g of the linear system (lane = row): H dux + rhs_g - dpi_{k-1} + A dpi_k + constraint multipliers
-FK_VLOOP
-            for (int i = li; i < nb; i += G) tmp0[i] = dlm[nb + i] - dlm[i];
-            double ap[RPM > 0 ? RPM : 1];
-            if (nx1 > 0) rows_dot<n, nx1>(MA, LDK, pik, ap);
-#pragma unroll
-            for (int m = 0; m < RP; m++)
-            {
-                const int i = li + G * m;
-                if (i < n)
-                {
-                    double r = hx[m] + gv[i];
-                    if (nx > 0 && i >= nu) r -= pim[i - nu];
-                    if (nx1 > 0) r += ap[m];
-                    g_[i] = r;
-                }
-            }
-            fk_sync();
-FK_VLOOP
-            for (int i = li; i < nb; i += G) g_[idxb[i]] += tmp0[i];
-            if (ns > 0)
-            {
-                const double *zv = gv + n;
-FK_VLOOP
-                for (int j = li; j < 2 * ns; j += G)
-                {
-                    double r = qZ[j] * dsv[j] + zv[j] - dlm[2 * nb + j];
-                    const int jj = j < ns ? j : j - ns, offl = j < ns ? 0 : nb;
-                    FK_FOR_SLACK(i, jj) r -= dlm[offl + i];
-                    g_[n + j] = r;
-                }
-            }
-            fk_sync();
-            double *og = v.w + sd.ires.g;
-FK_VLOOP
-            for (int i = li; i < n + 2 * ns; i += G)
-            {
-                const double r = g_[i];
-                if (so) og[i] = r;
-                const double a = fabs(r);
-                F.m0 = fmax(F.m0, a);
-                F.f0 |= (a != a);
-            }
-        }
-        FK_PROF_ADD2(22);      /* residual rows */
         if (nx1 > 0)
         {
 FK_VLOOP
-            for (int j = li; j < nx1; j += G)
-            {
-                vv[nu1 + j] = x1[j];
-                pim[j] = pik[j];
-            }
+            for (int j = li; j < nx1; j += G) vv[nu1 + j] = x1[j];
         }
     }
 
-    // returns the step length; lin_nrm = inf-norms of the residual of the linear system (do_lin)
+    // returns the step length; lin_nrm[1..3] = inf-norms of the b, d, m rows of the residual of the linear system (do_lin)
     FK_DEV double forward_pass(int after_fact, int do_lin, bool stw, double lin_nrm[4])
     {
         fk_fence_async_global();        // the records this sweep reads with bulk copies were written with plain stores by the sweeps before
 
         FwdAcc F;
         F.alpha = 1.0;
-        F.m0 = F.m1 = F.m2 = F.m3 = 0.0;
-        F.f0 = F.f1 = F.f2 = F.f3 = 0;
+        F.m1 = F.m2 = F.m3 = 0.0;
+        F.f1 = F.f2 = F.f3 = 0;
         fwd_stage<0>(0, after_fact, do_lin, stw, F);
         for (int k = 1; k < A.N; k++) fwd_stage<1>(k, after_fact, do_lin, stw, F);
         fwd_stage<2>(A.N, after_fact, do_lin, stw, F);
         if (do_lin)
         {
-            lin_nrm[0] = gmax_nan(F.m0, F.f0);
             lin_nrm[1] = gmax_nan(F.m1, F.f1);
             lin_nrm[2] = gmax_nan(F.m2, F.f2);
             lin_nrm[3] = gmax_nan(F.m3, F.f3);
@@ -1960,7 +2007,7 @@ FK_VLOOP
     // one interior-point iteration after pass kk: predictor / corrector / conditional corrector (OCP_QP_IPM_DELTA_STEP); leaves
     // the step length in Q.alpha.  Every sweep has exactly one call site (everything is inlined into the kernel, and the hot code
     // should exist once): the phases 0 / 1 / 2 of one inner loop.
-    FK_DEV void iteration(int q, int kk, QpState &Q, cuipm_info *info, double *stat)
+    FK_DEV void iteration(int q, int kk, QpState &Q, LinNrm &L, cuipm_info *info, double *stat)
     {
         const int SM = CUIPM_STAT_M;
         double *stt = (stat && kk + 1 < A.o.stat_max) ? stat + SM * (size_t) (kk + 1) : nullptr;
@@ -1975,17 +2022,11 @@ FK_VLOOP
             const int do_lin = ph == 0 ? A.o.lq_fact == 1 : A.o.itref_corr_max > 0;
             double nr[4] = {0, 0, 0, 0};
             double al; { FK_PROF_T0(); al = forward_pass(ph == 0, do_lin, stw, nr); FK_PROF_ADD(2); }
-            if (stw) { alpha = al; nrm[0] = nr[0]; nrm[1] = nr[1]; nrm[2] = nr[2]; nrm[3] = nr[3]; }
+            if (stw) { alpha = al; nrm[1] = nr[1]; nrm[2] = nr[2]; nrm[3] = nr[3]; }
             if (ph == 0)
             {
-                if (A.o.lq_fact == 1)
-                {
-                    // a Cholesky step that leaves a large residual in the linear system switches the solve to the LQ
-                    // refactorisation (x_ocp_qp_ipm.c:2246-2346): cold path, generic kernel
-                    const double g00 = (wk + A.s0.ires.g)[0];
-                    if ((nrm[0] == 0.0 && g00 != g00) || nrm[0] > 1e-5 || nrm[1] > 1e-5 || nrm[2] > 1e-5 || nrm[3] > 1e-5)
-                        if (act) { hand_back(q, info); act = false; }
-                }
+                // (the test itself waits for the stationarity rows: lin_check)
+                L.aff_bdm_large = nr[1] > 1e-5 || nr[2] > 1e-5 || nr[3] > 1e-5;
                 if (stt && act && li == 0) { stt[13] = 0; stt[0] = alpha; stt[1] = alpha; }
                 if (A.o.pred_corr != 1) break;
             }
@@ -2011,17 +2052,38 @@ FK_VLOOP
         {
             if (A.o.itref_corr_max > 0)
             {
-                // iterative refinement is needed when the residual of the corrector system is not small
-                // (x_ocp_qp_ipm.c:2540-2620): cold path, generic kernel
-                const bool small_ = (nrm[0] < A.o.res_g_max || nrm[0] < 1e-3 * Q.res_max[0]) && (nrm[1] < A.o.res_b_max || nrm[1] < 1e-3 * Q.res_max[1])
-                                    && (nrm[2] < A.o.res_d_max || nrm[2] < 1e-3 * Q.res_max[2]) && (nrm[3] < A.o.res_m_max || nrm[3] < 1e-3 * Q.res_max[3]);
-                if (!small_ && act) { hand_back(q, info); act = false; }
-                if (stt && act && li == 0) { stt[16] = nrm[0]; stt[17] = nrm[1]; stt[18] = nrm[2]; stt[19] = nrm[3]; }
+                // (the test itself waits for the stationarity rows: lin_check; stt[16] is written there)
+                L.res0_g = Q.res_max[0];
+                L.fin_bdm_small = (nrm[1] < A.o.res_b_max || nrm[1] < 1e-3 * Q.res_max[1]) && (nrm[2] < A.o.res_d_max || nrm[2] < 1e-3 * Q.res_max[2])
+                                  && (nrm[3] < A.o.res_m_max || nrm[3] < 1e-3 * Q.res_max[3]);
+                if (stt && act && li == 0) { stt[17] = nrm[1]; stt[18] = nrm[2]; stt[19] = nrm[3]; }
             }
             if (stt && act && li == 0) { stt[4] = alpha; stt[5] = alpha; }
         }
         if (stt && act && li == 0) stt[15] = 0;
         Q.alpha = alpha;
+    }
+
+    // the tests on the residual of the linear system of the iteration that led to pass kk, once the residual sweep of pass kk has
+    // formed its stationarity rows; a QP that fails one is handed back (it restarts from scratch in the generic kernel: the
+    // sweeps it ran here after the step that failed change none of its results)
+    FK_DEV void lin_check(int q, int kk, const LinNrm &L, cuipm_info *info, double *stat)
+    {
+        if (A.o.lq_fact == 1)
+        {
+            // a Cholesky step that leaves a large residual in the linear system switches the solve to the LQ
+            // refactorisation (x_ocp_qp_ipm.c:2246-2346): cold path, generic kernel
+            if (L.aff_g > 1e-5 || L.aff_bdm_large)
+                if (act) { hand_back(q, info); act = false; }
+        }
+        if (A.o.pred_corr == 1 && A.o.itref_corr_max > 0)
+        {
+            // iterative refinement is needed when the residual of the corrector system is not small
+            // (x_ocp_qp_ipm.c:2540-2620): cold path, generic kernel
+            const bool small_ = (L.fin_g < A.o.res_g_max || L.fin_g < 1e-3 * L.res0_g) && L.fin_bdm_small;
+            if (!small_ && act) { hand_back(q, info); act = false; }
+            if (stat && kk < A.o.stat_max && act && li == 0) stat[CUIPM_STAT_M * (size_t) kk + 16] = L.fin_g;
+        }
     }
 
     FK_DEV void solve(int q, bool valid)
@@ -2033,16 +2095,18 @@ FK_VLOOP
         QpState Q;
         Q.mu = Q.obj = Q.gap = 0.0; Q.alpha = 1.0; Q.res_m_tau = 0.0;
         Q.res_max[0] = Q.res_max[1] = Q.res_max[2] = Q.res_max[3] = 0.0;
+        LinNrm L;
         prologue(q, info, stat);
         // the residual sweep opens each pass of the loop (pass 0: residuals of the initial point; pass kk: move along the step
         // of iteration kk-1, then residuals)
         for (int kk = 0;; kk++)
         {
-            { FK_PROF_T0(); res_pass(kk > 0, Q.alpha, Q); FK_PROF_ADD(0); }
+            { FK_PROF_T0(); res_pass(kk > 0, Q.alpha, Q, L); FK_PROF_ADD(0); }
+            if (kk > 0) lin_check(q, kk, L, info, stat);
             close_pass(kk, Q, info, stat);
             // the warp leaves when none of its QPs continues
             if (!fk_any(act)) break;
-            iteration(q, kk, Q, info, stat);
+            iteration(q, kk, Q, L, info, stat);
         }
     }
 
@@ -2143,8 +2207,9 @@ FK_VLOOP
         QpState Q;
         Q.mu = Q.obj = Q.gap = 0.0; Q.alpha = 1.0; Q.res_m_tau = 0.0;
         Q.res_max[0] = Q.res_max[1] = Q.res_max[2] = Q.res_max[3] = 0.0;
+        LinNrm L;
         prologue(q, info, stat);
-        res_pass(0, 1.0, Q);
+        res_pass(0, 1.0, Q, L);
         close_pass(0, Q, info, stat);
         rr_publish(q, valid, 0, Q);
         fk_sync();
@@ -2210,11 +2275,13 @@ FK_VLOOP
             cuipm_info *info = A.info + q;
             double *stat = A.stat ? A.stat + (size_t) q * SM * (A.o.stat_max + 1) : nullptr;
             QpState Q;
+            LinNrm L;
             int kk = rr_load(q, Q);
             fk_sync();
-            iteration(q, kk, Q, info, stat);
+            iteration(q, kk, Q, L, info, stat);
             kk++;
-            { FK_PROF_T0(); res_pass(1, Q.alpha, Q); FK_PROF_ADD(0); }
+            { FK_PROF_T0(); res_pass(1, Q.alpha, Q, L); FK_PROF_ADD(0); }
+            lin_check(q, kk, L, info, stat);
             close_pass(kk, Q, info, stat);
             rr_publish(q, have, kk, Q);
         }
@@ -2237,11 +2304,11 @@ inline int vector_pool_doubles(int NX, int NM, int nce, int nbe, int ns2e, int n
 {
     const int nxe = (NX + 1) & ~1, nme = (NM + 2) & ~1;
     const int img = nve + nxe + 2 * nce;                                  // image of a (ux|g, pi|b, lam|d, t|m) record range
-    const int v_res = 2 * img + 2 * nme + (nxe + nme + 2 * nce + 2 * ns2e) + 2 * nbe + nve + 2 * nxe;
+    const int v_res = 2 * img + 2 * nme + (nxe + nme + 2 * nce + 2 * ns2e) + 2 * nbe + nve + 2 * nxe + (nve + nxe + nce);
     const int dd8 = 72 - (2 * nce + 2 * nbe + 2 * ns2e) > 0 ? 72 - (2 * nce + 2 * nbe + 2 * ns2e) : 0;
     const int v_fact = img + 2 * nce + ns2e + 2 * nce + 2 * nbe + 2 * ns2e + dd8 + 2 * nme + nxe + nme + nxe;
     const int v_slv = img + 2 * nce + (2 * nme + nxe + ns2e) + nce + 2 * nce + (nce + ns2e) + 2 * nce + 2 * nbe + ns2e + 2 * nxe;
-    const int v_fwd = img + 2 * nce + (2 * nme + nxe + ns2e) + nve + nme + (nce + ns2e) + nve + nxe + nve + 2 * nxe + 2 * nce + ns2e + nbe;
+    const int v_fwd = img + 2 * nce + (2 * nme + nxe + ns2e) + nve + nme + (nce + ns2e) + nve + nxe + nve + 2 * nce + ns2e;
     const int v_init = nve + nce, v_mu = 16 * nce;
     int m = v_res;
     if (v_mu > m) m = v_mu;

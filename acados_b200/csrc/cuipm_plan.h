@@ -142,6 +142,7 @@ inline bool fast_plan(const std::vector<StageDesc> &sd, const std::vector<int> &
         ok = ok && d.w_L == a.w_L + dw && d.w_Linv == a.w_Linv + dw && d.w_lrow == a.w_lrow + dw && d.w_Pb == a.w_Pb + dw && d.w_Zsi == a.w_Zsi + dw && d.w_Lxx == a.w_Lxx + dw
              && d.step.ux == a.step.ux + dw && d.step.pi == a.step.pi + dw && d.step.lam == a.step.lam + dw && d.step.t == a.step.t + dw
              && d.res.g == a.res.g + dw && d.res.b == a.res.b + dw && d.res.d == a.res.d + dw && d.res.m == a.res.m + dw && d.w_rmb == a.w_rmb + dw
+             && d.ires.g == a.ires.g + dw && d.ires.b == a.ires.b + dw && d.ires.d == a.ires.d + dw
              && d.itref.pi == a.itref.pi + dw && d.itref.lam == a.itref.lam + dw && d.itref.t == a.itref.t + dw;
         if (!ok) return false;
     }
