@@ -42,19 +42,7 @@ struct cuipm_solver
     int pending = 0;                         // an asynchronous host solve has been enqueued and not waited for
     float last_ms = 0.f;
     cuipm_opts last_opts{};
-    // throughput kernel (cuipm_fast.cu)
-    bool fast_ok = false;
-    int use_fast = 1;                        // tuning key "fast"
-    int fast_qpw = 1;
-    FastArgs F{};
-    int *d_redo_list = nullptr, *d_redo_count = nullptr;
-    // iteration-sliced scheduling of the throughput kernel (tuning key "rr"): per-QP scalar state, ring, counters per chunk
-    bool rr_ok = false;
-    int use_rr = 1;                          // tuning key "rr": 0 off, 1 when the batch exceeds the resident QPs, 2 always
-    int rr_resident = 0;
-    double *d_rr_state = nullptr;
-    int *d_rr_ring = nullptr, *d_rr_ctr = nullptr;
-    double *d_qpk = nullptr;                 // kernel-side QP records (repack pass)
+    FastPath fast;                           // throughput kernel (cuipm_fast.cu)
     cudaEvent_t evk0 = nullptr, evk1 = nullptr;   // around the throughput kernel of the last cuipm_solve_device call
     bool timed_fast = false;
 };
@@ -80,24 +68,7 @@ static int build_desc(cuipm_solver *s, const cuipm_shape *sh)
     CK(cudaMemcpy(s->d_sd, s->sd_host.data(), sizeof(StageDesc) * (N + 1), cudaMemcpyHostToDevice));
     CK(cudaMalloc(&s->d_ipool, sizeof(int) * (ipool.size() + 1)));
     if (!ipool.empty()) CK(cudaMemcpy(s->d_ipool, ipool.data(), sizeof(int) * ipool.size(), cudaMemcpyHostToDevice));
-    // throughput kernel: eligible shape with a compiled instance
-    s->fast_ok = fast_plan(s->sd_host, ipool, s->P, s->F) && fast_available(s->F.s1.nx, s->F.s1.nu, s->F, &s->fast_qpw);
-    if (s->fast_ok)
-    {
-        CK(cudaMalloc(&s->d_redo_list, sizeof(int) * (size_t) s->max_batch));
-        CK(cudaMalloc(&s->d_redo_count, sizeof(int) * 2 * cuipm_solver::kPipe));      // hand-back counter + work counter per chunk
-        CK(cudaMemset(s->d_redo_count, 0, sizeof(int) * 2 * cuipm_solver::kPipe));
-        CK(cudaMalloc(&s->d_qpk, sizeof(double) * s->F.qpk_stride * (size_t) s->max_batch));
-        CK(cudaMemset(s->d_qpk, 0, sizeof(double) * s->F.qpk_stride * (size_t) s->max_batch));
-        s->rr_ok = fast_rr_available(s->F.s1.nx, s->F.s1.nu);
-        if (s->rr_ok)
-        {
-            CK(cudaMalloc(&s->d_rr_state, sizeof(double) * 12 * (size_t) s->max_batch));
-            CK(cudaMalloc(&s->d_rr_ring, sizeof(int) * CUIPM_RR_RINGS * (size_t) s->max_batch));
-            CK(cudaMalloc(&s->d_rr_ctr, sizeof(int) * CUIPM_RR_CTR * cuipm_solver::kPipe));
-        }
-    }
-    return CUIPM_OK;
+    return s->fast.create(s->sd_host, ipool, s->P, s->max_batch, cuipm_solver::kPipe, s->device);
 }
 
 // One batch (or one chunk of it) on `stream`: the throughput kernel where the shape and the options allow it, then the
@@ -108,43 +79,11 @@ static int launch_batch(cuipm_solver *s, const LaunchArgs &a0, int slot, size_t 
     LaunchArgs a = a0;
     a.redo_list = nullptr;
     a.redo_count = nullptr;
-    const cuipm_opts &o = a.o;
-    // (m != 0 -- acados' tau_min option -- changes the ratio test into the quadratic rule: generic kernel only, the hot code of
-    // the throughput kernel stays as it is)
-    if (s->fast_ok && s->use_fast && o.lq_fact <= 1 && o.m_relax == 0.0 && !(((size_t) a.sol | (size_t) a.work) & 15))
-    {
-        FastArgs F = s->F;
-        F.nbatch = a.nbatch; F.ipool = a.ipool; F.qp = a.qp; F.sol = a.sol; F.work = a.work; F.info = a.info; F.stat = a.stat;
-        F.qpk = s->d_qpk + s->F.qpk_stride * lo;
-        F.redo_list = s->d_redo_list + lo; F.redo_count = s->d_redo_count + 2 * slot; F.next_qp = F.redo_count + 1; F.o = o;
-        cudaError_t e = cudaMemsetAsync(F.redo_count, 0, 2 * sizeof(int), stream);
-        if (e != cudaSuccess) { set_error(std::string("cudaMemsetAsync: ") + cudaGetErrorString(e)); return CUIPM_ERR_CUDA; }
-        int rc = launch_repack(F, s->d_sd, (void *) stream);
-        if (rc != 0) { set_error(std::string("kernel launch (repack): ") + cudaGetErrorString((cudaError_t) rc)); return CUIPM_ERR_CUDA; }
-        (*launches)++;
-        if (slot == 0 && s->evk0) cudaEventRecord(s->evk0, stream);
-        // iteration-sliced scheduling pays when the batch is more than one wave of resident QPs and not many; small batches keep the
-        // single launch (below one wave the extra launch and the ring traffic cost more than the idle slots they save)
-        if (s->rr_ok && s->rr_resident == 0) s->rr_resident = fast_resident_qps(F) > 0 ? fast_resident_qps(F) : -1;
-        const bool rr = s->rr_ok && s->use_rr && (s->use_rr > 1 || (s->rr_resident > 0 && a.nbatch > s->rr_resident));
-        if (rr)
-        {
-            F.rr_state = s->d_rr_state + 12 * lo; F.rr_ring = s->d_rr_ring + CUIPM_RR_RINGS * lo; F.rr_ctr = s->d_rr_ctr + CUIPM_RR_CTR * slot;
-            e = cudaMemsetAsync(F.rr_ring, 0xff, sizeof(int) * CUIPM_RR_RINGS * (size_t) a.nbatch, stream);
-            if (e == cudaSuccess) e = cudaMemsetAsync(F.rr_ctr, 0, CUIPM_RR_CTR * sizeof(int), stream);
-            if (e != cudaSuccess) { set_error(std::string("cudaMemsetAsync: ") + cudaGetErrorString(e)); return CUIPM_ERR_CUDA; }
-            rc = launch_fast(F, (void *) stream, 1);
-            if (rc == 0) { (*launches)++; rc = launch_fast(F, (void *) stream, 2); }
-        }
-        else
-            rc = launch_fast(F, (void *) stream, 0);
-        if (slot == 0 && s->evk1) { cudaEventRecord(s->evk1, stream); s->timed_fast = true; }
-        if (rc != 0) { set_error(std::string("kernel launch (throughput kernel): ") + cudaGetErrorString((cudaError_t) rc)); return CUIPM_ERR_CUDA; }
-        (*launches)++;
-        a.redo_list = F.redo_list;
-        a.redo_count = F.redo_count;
-    }
-    int rc = launch_solve(a, s->warps, (void *) stream);
+    const bool timed = slot == 0 && s->evk0;
+    int rc = s->fast.enqueue(a, lo, slot, (void *) stream, launches, timed ? s->evk0 : nullptr, timed ? s->evk1 : nullptr);
+    if (rc != CUIPM_OK) return rc;
+    if (timed && a.redo_count) s->timed_fast = true;
+    rc = launch_solve(a, s->warps, (void *) stream);
     if (rc != 0) { set_error(std::string("kernel launch: ") + cudaGetErrorString((cudaError_t) rc)); return CUIPM_ERR_CUDA; }
     (*launches)++;
     return CUIPM_OK;
@@ -198,8 +137,7 @@ extern "C" void cuipm_destroy(cuipm_solver *s)
     if (s->stream) cudaStreamSynchronize(s->stream);
     cudaFree(s->d_sd); cudaFree(s->d_ipool); cudaFree(s->d_qp); cudaFree(s->d_sol); cudaFree(s->d_work);
     cudaFree(s->d_stat); cudaFree(s->d_info); cudaFree(s->d_seed); cudaFree(s->d_sens);
-    cudaFree(s->d_redo_list); cudaFree(s->d_redo_count); cudaFree(s->d_qpk);
-    cudaFree(s->d_rr_state); cudaFree(s->d_rr_ring); cudaFree(s->d_rr_ctr);
+    s->fast.destroy();
     if (s->ev0) cudaEventDestroy(s->ev0);
     if (s->ev1) cudaEventDestroy(s->ev1);
     if (s->evk0) cudaEventDestroy(s->evk0);
@@ -230,13 +168,10 @@ extern "C" void *cuipm_stream(cuipm_solver *s) { return (void *) s->stream; }
 extern "C" int cuipm_last_launch_count(const cuipm_solver *s) { return s->last_launches; }
 extern "C" int cuipm_last_handed_back(cuipm_solver *s)
 {
-    if (!s || !s->fast_ok || !s->d_redo_count) return 0;
-    int total = 0, h[2 * cuipm_solver::kPipe];
+    if (!s || !s->fast.inst) return 0;
     cudaSetDevice(s->device);
     cudaStreamSynchronize(s->stream);
-    if (cudaMemcpy(h, s->d_redo_count, sizeof(h), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
-    for (int c = 0; c < cuipm_solver::kPipe; c++) total += h[2 * c];
-    return total;
+    return s->fast.handed_back();
 }
 extern "C" float cuipm_last_main_kernel_ms(cuipm_solver *s)
 {
@@ -262,12 +197,12 @@ extern "C" int cuipm_set_tuning(cuipm_solver *s, const char *key, int value)
     }
     if (!std::strcmp(key, "rr"))
     {
-        s->use_rr = value;
+        s->fast.rr = value;
         return CUIPM_OK;
     }
     if (!std::strcmp(key, "fast"))
     {
-        s->use_fast = value != 0;
+        s->fast.use = value != 0;
         return CUIPM_OK;
     }
     set_error("unknown tuning key");

@@ -3,6 +3,7 @@
 #define CUIPM_DEVICE_H_
 
 #include <cstddef>
+#include <vector>
 
 #include "cuipm.h"
 
@@ -119,22 +120,44 @@ struct FastArgs
 
 // launches the solve kernel with `warps` warps per QP on `stream`; returns cudaError_t as int
 int launch_solve(const LaunchArgs &a, int warps, void *stream);
-// throughput path: true if a kernel instance exists for interior (nx, nu); fills the shared-memory figures of F
-bool fast_available(int nx, int nu, FastArgs &F, int *qp_per_warp);
-// caller's QP records -> kernel-side records (F.qpk) for F.nbatch QPs on `stream`; sd = device stage table; returns cudaError_t as int
-int launch_repack(const FastArgs &F, const StageDesc *sd, void *stream);
-// launches the throughput kernel for F on `stream`; returns cudaError_t as int.  mode 0: a QP stays with its warp; 1 then 2: the two
-// launches of the iteration-sliced scheduling (fast_rr_available says whether the instance has them)
-int launch_fast(const FastArgs &F, void *stream, int mode);
-bool fast_rr_available(int nx, int nu);
-// QPs the device holds at once with the throughput kernel of F's shape (0 if unknown)
-int fast_resident_qps(const FastArgs &F);
 // launches the sensitivity kernel (one substitution with the factorisation the last solve left in the work records)
 int launch_sens(const LaunchArgs &a, int warps, void *stream);
-// dynamic shared memory (bytes) the kernel needs for P
-size_t smem_bytes(const ProbDesc &P);
-// largest warps-per-QP value compiled
-int max_warps();
+
+struct FastInstance;   // compiled instance of the throughput kernel (cuipm_fast.cu)
+
+// The throughput path of one solver (cuipm_fast.cu): the plan of its shape, the kernel instance that runs it, the buffers the
+// kernel needs besides the solver's records, and the choice of schedule.  Streams and events are cudaStream_t / cudaEvent_t
+// passed as void *, so that host-only code can include this header.
+struct FastPath
+{
+    const FastInstance *inst = nullptr;   // null: the shape has no throughput kernel
+    FastArgs F{};                         // plan of the shape; enqueue adds the records of each batch
+    size_t smem = 0;                      // dynamic shared memory per CTA (bytes)
+    int sms = 1;                          // SMs of the solver's device
+    int ctas[3] = {1, 1, 1};              // CTAs the device holds at once with this shared memory, per launch mode
+    int ring_qps = 0;                     // QPs the device holds at once in mode 0 (0: unknown)
+    int nslot = 0;                        // chunks that may run concurrently (one set of counters each)
+    int use = 1;                          // tuning key "fast": 0 off
+    int rr = 1;                           // tuning key "rr": iteration-sliced scheduling 0 off, 1 when the batch exceeds ring_qps, 2 always
+    double *qpk = nullptr;                // kernel-side QP records (repack pass)
+    int *redo_list = nullptr;             // QPs handed back to the generic kernel
+    int *ctr = nullptr;                   // per slot: hand-back count, work counter of the persistent warps
+    double *rr_state = nullptr;           // iteration-sliced scheduling: per-QP scalar state, rings, ring counters per slot
+    int *rr_ring = nullptr, *rr_ctr = nullptr;
+
+    // Plans the shape of sd / ipool / P and, if a kernel instance runs it, sizes its shared memory, allocates the buffers for
+    // max_batch QPs in nslot concurrent chunks and measures the residency on `device` (the current device).  Returns CUIPM_OK
+    // (inst stays null for a shape without a throughput kernel) or an error code with the message set.
+    int create(const std::vector<StageDesc> &sd, const std::vector<int> &ipool, const ProbDesc &P, int max_batch, int nslot, int device);
+    // One batch or chunk `a` (QPs lo .. lo + a.nbatch - 1 of the solver's buffers, counters of `slot`) on `stream`, if the path
+    // takes it (shape, options, 16-byte aligned records): repack, then the throughput kernel; ev_repacked / ev_done, if not null,
+    // are recorded after the repack and after the last throughput-kernel launch.  Sets a.redo_list / a.redo_count to the QPs
+    // handed back and adds to *launches; leaves `a` as it is if the path does not take the batch.  Returns CUIPM_OK or an error.
+    int enqueue(LaunchArgs &a, size_t lo, int slot, void *stream, int *launches, void *ev_repacked, void *ev_done);
+    // QPs handed back by the last batch or chunks (inst not null, the solver's streams idle); -1 on error
+    int handed_back() const;
+    void destroy();
+};
 
 }  // namespace cuipm
 #endif

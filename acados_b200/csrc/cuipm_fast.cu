@@ -3,16 +3,18 @@
 // The kernel body is cuipm_fast_core.h (a group of G lanes per QP, 32/G QPs per warp in lock step, register-tiled
 // rank-k updates, stage blocks staged with asynchronous copies); this file binds its warp primitives to the hardware
 // (shuffles, votes, cp.async, __syncwarp) and launches one warp per CTA, 32/G QPs per CTA.  Replaces, for the shapes
-// listed in fast_available(), the reference's d_ocp_qp_ipm_solve (external/hpipm/ocp_qp/x_ocp_qp_ipm.c:2684-3120) on
+// in CUIPM_FAST_INSTANCES below, the reference's d_ocp_qp_ipm_solve (external/hpipm/ocp_qp/x_ocp_qp_ipm.c:2684-3120) on
 // BLASFEO's panel-major kernels (dsyrk_dpotrf_ln_mn, dtrmm_rlnn: external/blasfeo/blasfeo_hp_pm/d_lapack_lib4.c:1513,
-// d_blas3_lib4.c:4893).
+// d_blas3_lib4.c:4893).  The host side of the throughput path (FastPath, cuipm_device.h) is at the end of this file.
 #include <cuda_runtime.h>
 
 #include <cmath>
-#include <cstdio>
-#include <cstdlib>
+#include <string>
+#include <vector>
 
 #include "cuipm_device.h"
+#include "cuipm_internal.h"
+#include "cuipm_plan.h"
 
 #define FK_DEV __device__ __forceinline__
 static __device__ __forceinline__ int fk_lane() { return (int) (threadIdx.x & 31u); }
@@ -42,17 +44,6 @@ static __device__ __forceinline__ void fk_bulk(double *sdst, const double *gsrc,
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(sa), "l"(gsrc), "r"(bytes), "r"(ba)
                  : "memory");
 }
-// the same range of the records of the n QPs of a warp (record stride rstep; the groups beyond nvalid re-read the last one) into
-// the n groups' shared memory (group stride gstride doubles); kept out of line
-static __device__ __noinline__ void fk_bulk_groups(double *sdst, const double *gsrc, unsigned bytes, fk_mbar_t *b, int n, int gstride, size_t rstep, int nvalid)
-{
-    for (int g = 0; g < n; g++)
-    {
-        fk_bulk(sdst, gsrc, bytes, b);
-        sdst += gstride;
-        if (g + 1 < nvalid) gsrc += rstep;
-    }
-}
 static __device__ __forceinline__ void fk_mbar_arrive_tx(fk_mbar_t *b, unsigned bytes)
 {
     const unsigned ba = (unsigned) __cvta_generic_to_shared(b);
@@ -69,11 +60,6 @@ static __device__ __forceinline__ void fk_mbar_wait(fk_mbar_t *b, unsigned parit
         "bra WAIT_%=;\n\t"
         "DONE_%=:\n\t}" ::"r"(ba), "r"(parity)
         : "memory");
-}
-// L2 prefetch of a contiguous range (TMA bulk prefetch): no destination, no completion
-static __device__ __forceinline__ void fk_prefetch_l2(const double *gsrc, unsigned bytes)
-{
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gsrc), "r"(bytes) : "memory");
 }
 // orders this thread's earlier generic-proxy accesses to shared memory before later asynchronous-proxy (bulk copy) writes to it
 static __device__ __forceinline__ void fk_fence_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -124,12 +110,12 @@ template <int NX, int NU, int G, int MINB, int MODE>
 __global__ void __launch_bounds__(32, MINB) cuipm_fast_kernel(const __grid_constant__ FastArgs A)
 {
     using K = fastk::Ker<NX, NU, G>;
-    __shared__ __align__(8) fk_mbar_t bars[6];
+    __shared__ __align__(8) fk_mbar_t bar;
 #ifdef FK_PROFILE
     if (fk_lane() == 0) for (int i = 0; i < 32; i++) g_prof[i] = 0;
     const long long tk0 = clock64();
 #endif
-    K k(A, g_fsmem, bars);
+    K k(A, g_fsmem, &bar);
     // persistent warps: each one fetches the next 32/G QPs of the batch until none is left (QPs need 6..18 iterations, and
     // a launch is a few waves of resident warps: a fixed assignment leaves SMs idle at the end of every wave)
     if (MODE == 2)
@@ -185,55 +171,9 @@ __global__ void __launch_bounds__(256) cuipm_repack_kernel(const FastArgs A, con
     }
 }
 
-template <int NX, int NU, int G>
-void sizes(FastArgs &F, int *qpw)
-{
-    using K = fastk::Ker<NX, NU, G>;
-    F.vsize = fastk::vector_pool_doubles(NX, NX + NU, F.nce, F.nbe, F.ns2e, F.nve);
-    int gs = K::MATS + F.vsize;
-    // 32 / G groups share a warp; 64-bit shared loads are served per half-warp: a group stride of 8 (mod 16) doubles puts the
-    // consecutive-row accesses of the two groups of a half-warp on disjoint banks
-    while (gs % 16 != 8) gs++;
-    F.gstride = gs;
-    *qpw = K::QPW;
-}
-
-template <int NX, int NU, int G, int MINB, int MODE>
-cudaError_t launch_one(const FastArgs &F, cudaStream_t stream)
-{
-    using K = fastk::Ker<NX, NU, G>;
-    const size_t smem = sizeof(double) * ((size_t) F.gstride * K::QPW + 2 * (size_t) F.nmaps * F.nbe);
-    if (((size_t) F.qpk | (size_t) F.sol | (size_t) F.work) & 15) return cudaErrorMisalignedAddress;      // bulk copies need 16-byte aligned records
-    cudaError_t err = cudaFuncSetAttribute(cuipm_fast_kernel<NX, NU, G, MINB, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-    if (err != cudaSuccess) return err;
-    // the CTAs of one SM together need most of its shared memory: ask for the largest carve-out (the default heuristic
-    // sized it for a single CTA, which left one warp per SM resident)
-    err = cudaFuncSetAttribute(cuipm_fast_kernel<NX, NU, G, MINB, MODE>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (err != cudaSuccess) return err;
-    if (getenv("CUIPM_DEBUG"))
-    {
-        int nblk = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, cuipm_fast_kernel<NX, NU, G, MINB, MODE>, 32, smem);
-        fprintf(stderr, "cuipm_fast_kernel<%d,%d,%d>: %zu bytes of shared memory per CTA, %d CTAs (%d QPs) per SM\n", NX, NU, G, smem, nblk, nblk * K::QPW);
-    }
-    static int resident = 0;        // CTAs per SM x SMs of this instance
-    if (!resident)
-    {
-        int nblk = 0, dev = 0, sms = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, cuipm_fast_kernel<NX, NU, G, MINB, MODE>, 32, smem);
-        resident = (nblk > 0 ? nblk : 1) * (sms > 0 ? sms : 1);
-    }
-    const int want = (F.nbatch + K::QPW - 1) / K::QPW;
-    const int grid = want < resident ? want : resident;       // (the ring loop too: more warps than QP groups would only poll)
-    cuipm_fast_kernel<NX, NU, G, MINB, MODE><<<grid, 32, smem, stream>>>(F);
-    return cudaGetLastError();
-}
-
 }  // namespace
 
-// (interior nx, nu) pairs with an instance of the throughput kernel, and the lanes per QP each one runs with
+// the compiled instances: interior (nx, nu), lanes per QP, minimum CTAs per SM of the launch bounds
 #define CUIPM_FAST_INSTANCES(X) \
     X(21, 3, 8, 4)              \
     X(8, 3, 4, 8)               \
@@ -241,43 +181,138 @@ cudaError_t launch_one(const FastArgs &F, cudaStream_t stream)
     X(12, 4, 8, 6)              \
     X(48, 12, 32, 3)
 
-// development: other lanes-per-QP mappings of the headline shape, selected with CUIPM_FAST_G=16|32
-#ifdef CUIPM_FAST_DEV
-#define CUIPM_FAST_DEV_INSTANCES(X) \
-    X(21, 3, 16, 8)                 \
-    X(21, 3, 32, 16)
-#else
-#define CUIPM_FAST_DEV_INSTANCES(X)
-#endif
-static int dev_g() { const char *e = getenv("CUIPM_FAST_G"); return e ? atoi(e) : 0; }
+typedef void (*FastKernel)(FastArgs);
 
-bool fast_available(int nx, int nu, FastArgs &F, int *qp_per_warp)
+// one instance: the interior (nx, nu) it runs, QPs per warp, its shared-memory layout (cuipm_fast_core.h) and its kernels for
+// launch mode 0 (a QP stays with its warp), 1 and 2 (iteration-sliced scheduling: initial points and ring filled, loop over the ring)
+struct FastInstance
 {
+    int nx, nu, qpw;
+    size_t (*layout)(FastArgs &);
+    FastKernel kernel[3];
+};
+
+static const FastInstance kInstances[] = {
 #define X(NX_, NU_, G_, MB_) \
-    if (nx == NX_ && nu == NU_ && dev_g() == G_) { sizes<NX_, NU_, G_>(F, qp_per_warp); return sizeof(double) * ((size_t) F.gstride * (32 / G_) + 2 * (size_t) F.nmaps * F.nbe) <= 226 * 1024; }
-    CUIPM_FAST_DEV_INSTANCES(X)
-#undef X
-#define X(NX_, NU_, G_, MB_) \
-    if (nx == NX_ && nu == NU_) { sizes<NX_, NU_, G_>(F, qp_per_warp); return sizeof(double) * ((size_t) F.gstride * (32 / G_) + 2 * (size_t) F.nmaps * F.nbe) <= 226 * 1024; }
+    {NX_, NU_, 32 / G_, fastk::layout<NX_, NU_, G_>, {cuipm_fast_kernel<NX_, NU_, G_, MB_, 0>, cuipm_fast_kernel<NX_, NU_, G_, MB_, 1>, cuipm_fast_kernel<NX_, NU_, G_, MB_, 2>}},
     CUIPM_FAST_INSTANCES(X)
 #undef X
-    return false;
+};
+
+#define CKF(what, call)                                                                                 \
+    do {                                                                                                \
+        cudaError_t e_ = (call);                                                                        \
+        if (e_ != cudaSuccess)                                                                          \
+        {                                                                                               \
+            set_error(std::string(what) + ": " + cudaGetErrorString(e_));                               \
+            return CUIPM_ERR_CUDA;                                                                      \
+        }                                                                                               \
+    } while (0)
+
+// The dynamic shared memory attribute belongs to the kernel, not to a solver: solvers of other shapes may launch the same
+// instance with more, so it is set before every launch.  The CTAs of one SM together need most of its shared memory: ask for
+// the largest carve-out (the default heuristic sized it for a single CTA, which left one warp per SM resident).
+static cudaError_t set_smem(FastKernel k, size_t smem)
+{
+    cudaError_t err = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+    if (err == cudaSuccess) err = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    return err;
 }
 
-int launch_repack(const FastArgs &F, const StageDesc *sd, void *stream_)
+int FastPath::create(const std::vector<StageDesc> &sd, const std::vector<int> &ipool, const ProbDesc &P, int max_batch, int nslot_, int device)
 {
-    cudaStream_t stream = (cudaStream_t) stream_;
-    static int sms = 0;
-    if (!sms)
+    if (!fast_plan(sd, ipool, P, F)) return CUIPM_OK;
+    const FastInstance *in = nullptr;
+    for (const FastInstance &i : kInstances)
+        if (i.nx == F.s1.nx && i.nu == F.s1.nu) in = &i;
+    if (!in) return CUIPM_OK;
+    smem = in->layout(F);
+    if (smem > 226 * 1024) return CUIPM_OK;
+    inst = in;
+    nslot = nslot_;
+    const size_t nb = (size_t) max_batch;
+    CKF("cudaMalloc", cudaMalloc(&redo_list, sizeof(int) * nb));
+    CKF("cudaMalloc", cudaMalloc(&ctr, sizeof(int) * 2 * nslot));
+    CKF("cudaMemset", cudaMemset(ctr, 0, sizeof(int) * 2 * nslot));
+    CKF("cudaMalloc", cudaMalloc(&qpk, sizeof(double) * F.qpk_stride * nb));
+    CKF("cudaMemset", cudaMemset(qpk, 0, sizeof(double) * F.qpk_stride * nb));
+    CKF("cudaMalloc", cudaMalloc(&rr_state, sizeof(double) * 12 * nb));
+    CKF("cudaMalloc", cudaMalloc(&rr_ring, sizeof(int) * CUIPM_RR_RINGS * nb));
+    CKF("cudaMalloc", cudaMalloc(&rr_ctr, sizeof(int) * CUIPM_RR_CTR * nslot));
+    // residency with this solver's shared memory, per mode (the three kernels need different numbers of registers)
+    CKF("cudaDeviceGetAttribute", cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+    for (int m = 0; m < 3; m++)
     {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        if (sms <= 0) sms = 1;
+        int nblk = 0;
+        CKF("cudaFuncSetAttribute", set_smem(inst->kernel[m], smem));
+        CKF("cudaOccupancyMaxActiveBlocksPerMultiprocessor", cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, inst->kernel[m], 32, smem));
+        ctas[m] = (nblk > 0 ? nblk : 1) * sms;
+        if (m == 0) ring_qps = nblk * sms * inst->qpw;
     }
-    const int grid = F.nbatch < sms * 8 ? F.nbatch : sms * 8;      // eight CTAs per SM, grid-stride over the batch
-    cuipm_repack_kernel<<<grid, 256, 0, stream>>>(F, sd);
-    return (int) cudaGetLastError();
+    return CUIPM_OK;
+}
+
+// the throughput kernel of `mode` over f.nbatch QPs: persistent warps, at most as many CTAs as the device holds at once (the
+// ring loop too: more warps than QP groups would only poll)
+static cudaError_t launch(const FastPath &p, int mode, const FastArgs &f, cudaStream_t stream)
+{
+    const FastKernel k = p.inst->kernel[mode];
+    cudaError_t err = set_smem(k, p.smem);
+    if (err != cudaSuccess) return err;
+    const int want = (f.nbatch + p.inst->qpw - 1) / p.inst->qpw;
+    k<<<want < p.ctas[mode] ? want : p.ctas[mode], 32, p.smem, stream>>>(f);
+    return cudaGetLastError();
+}
+
+int FastPath::enqueue(LaunchArgs &a, size_t lo, int slot, void *stream_, int *launches, void *ev_repacked, void *ev_done)
+{
+    // (m != 0 -- acados' tau_min option -- changes the ratio test into the quadratic rule: generic kernel only, the hot code of
+    // the throughput kernel stays as it is; the bulk copies need 16-byte aligned records)
+    if (!inst || !use || a.o.lq_fact > 1 || a.o.m_relax != 0.0 || (((size_t) a.sol | (size_t) a.work) & 15)) return CUIPM_OK;
+    cudaStream_t stream = (cudaStream_t) stream_;
+    FastArgs f = F;
+    f.nbatch = a.nbatch; f.ipool = a.ipool; f.qp = a.qp; f.sol = a.sol; f.work = a.work; f.info = a.info; f.stat = a.stat; f.o = a.o;
+    f.qpk = qpk + F.qpk_stride * lo;
+    f.redo_list = redo_list + lo; f.redo_count = ctr + 2 * slot; f.next_qp = f.redo_count + 1;
+    CKF("cudaMemsetAsync", cudaMemsetAsync(f.redo_count, 0, 2 * sizeof(int), stream));
+    cuipm_repack_kernel<<<f.nbatch < sms * 8 ? f.nbatch : sms * 8, 256, 0, stream>>>(f, a.sd);      // eight CTAs per SM, grid-stride over the batch
+    CKF("kernel launch (repack)", cudaGetLastError());
+    (*launches)++;
+    if (ev_repacked) cudaEventRecord((cudaEvent_t) ev_repacked, stream);
+    // iteration-sliced scheduling pays when the batch is more than one wave of resident QPs and not many; small batches keep the
+    // single launch (below one wave the extra launch and the ring traffic cost more than the idle slots they save)
+    cudaError_t e;
+    if (rr && (rr > 1 || (ring_qps > 0 && a.nbatch > ring_qps)))
+    {
+        f.rr_state = rr_state + 12 * lo; f.rr_ring = rr_ring + CUIPM_RR_RINGS * lo; f.rr_ctr = rr_ctr + CUIPM_RR_CTR * slot;
+        CKF("cudaMemsetAsync", cudaMemsetAsync(f.rr_ring, 0xff, sizeof(int) * CUIPM_RR_RINGS * (size_t) a.nbatch, stream));
+        CKF("cudaMemsetAsync", cudaMemsetAsync(f.rr_ctr, 0, CUIPM_RR_CTR * sizeof(int), stream));
+        e = launch(*this, 1, f, stream);
+        if (e == cudaSuccess) { (*launches)++; e = launch(*this, 2, f, stream); }
+    }
+    else
+        e = launch(*this, 0, f, stream);
+    if (ev_done) cudaEventRecord((cudaEvent_t) ev_done, stream);
+    CKF("kernel launch (throughput kernel)", e);
+    (*launches)++;
+    a.redo_list = f.redo_list;
+    a.redo_count = f.redo_count;
+    return CUIPM_OK;
+}
+
+int FastPath::handed_back() const
+{
+    std::vector<int> h(2 * nslot);
+    if (cudaMemcpy(h.data(), ctr, sizeof(int) * h.size(), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+    int total = 0;
+    for (int c = 0; c < nslot; c++) total += h[2 * c];
+    return total;
+}
+
+void FastPath::destroy()
+{
+    cudaFree(qpk); cudaFree(redo_list); cudaFree(ctr);
+    cudaFree(rr_state); cudaFree(rr_ring); cudaFree(rr_ctr);
 }
 
 #ifdef FK_PROFILE
@@ -288,66 +323,5 @@ extern "C" void cuipm_fast_prof_read(unsigned long long *out, int reset)
     if (reset) { unsigned long long z[32] = {0}; cudaMemcpyToSymbol(cuipm_fast_prof, z, sizeof(z)); }
 }
 #endif
-
-// instances with the iteration-sliced scheduling compiled in (two more kernels each)
-#define CUIPM_FAST_RR_INSTANCES(X) CUIPM_FAST_INSTANCES(X)
-
-// QPs the device holds at once with the throughput kernel of this shape (CTAs per SM x SMs x QPs per warp); 0 if unknown
-template <int NX, int NU, int G, int MINB>
-static int resident_qps(const FastArgs &F)
-{
-    using K = fastk::Ker<NX, NU, G>;
-    const size_t smem = sizeof(double) * ((size_t) F.gstride * K::QPW + 2 * (size_t) F.nmaps * F.nbe);
-    int nblk = 0, dev = 0, sms = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaFuncSetAttribute(cuipm_fast_kernel<NX, NU, G, MINB, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-    cudaFuncSetAttribute(cuipm_fast_kernel<NX, NU, G, MINB, 0>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, cuipm_fast_kernel<NX, NU, G, MINB, 0>, 32, smem) != cudaSuccess) return 0;
-    return nblk * sms * K::QPW;
-}
-
-int fast_resident_qps(const FastArgs &F)
-{
-    const int nx = F.s1.nx, nu = F.s1.nu;
-#define X(NX_, NU_, G_, MB_) \
-    if (nx == NX_ && nu == NU_) return resident_qps<NX_, NU_, G_, MB_>(F);
-    CUIPM_FAST_INSTANCES(X)
-#undef X
-    return 0;
-}
-
-bool fast_rr_available(int nx, int nu)
-{
-    if (dev_g()) return false;
-#define X(NX_, NU_, G_, MB_) \
-    if (nx == NX_ && nu == NU_) return true;
-    CUIPM_FAST_RR_INSTANCES(X)
-#undef X
-    return false;
-}
-
-int launch_fast(const FastArgs &F, void *stream_, int mode)
-{
-    cudaStream_t stream = (cudaStream_t) stream_;
-    const int nx = F.s1.nx, nu = F.s1.nu;
-    if (mode != 0)
-    {
-#define X(NX_, NU_, G_, MB_) \
-        if (nx == NX_ && nu == NU_) return (int) (mode == 1 ? launch_one<NX_, NU_, G_, MB_, 1>(F, stream) : launch_one<NX_, NU_, G_, MB_, 2>(F, stream));
-        CUIPM_FAST_RR_INSTANCES(X)
-#undef X
-        return (int) cudaErrorInvalidValue;
-    }
-#define X(NX_, NU_, G_, MB_) \
-    if (nx == NX_ && nu == NU_ && dev_g() == G_) return (int) launch_one<NX_, NU_, G_, MB_, 0>(F, stream);
-    CUIPM_FAST_DEV_INSTANCES(X)
-#undef X
-#define X(NX_, NU_, G_, MB_) \
-    if (nx == NX_ && nu == NU_) return (int) launch_one<NX_, NU_, G_, MB_, 0>(F, stream);
-    CUIPM_FAST_INSTANCES(X)
-#undef X
-    return (int) cudaErrorInvalidValue;
-}
 
 }  // namespace cuipm

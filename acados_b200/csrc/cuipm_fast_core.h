@@ -6,10 +6,11 @@
 // of (row slots) x 8 columns fed by one LDS per own row and 128-bit broadcast loads of the other operand; the gradient
 // travels as a vector next to the factorisation (a fused right-looking substitution), so the row slots hold matrix rows only.
 //
-// Data movement: every input of a stage -- the dynamics block, the Hessian block, the factor of the next stage and the
-// "images" of the contiguous vector ranges of the three records -- is brought into shared memory by bulk asynchronous
-// copies (TMA, cp.async.bulk) issued by one lane with warp-uniform operands and completed on an mbarrier; the arithmetic
-// then runs on shared memory and registers only, results leave through plain stores.  The matrices come from the
+// Data movement: every input of a stage is brought into shared memory by asynchronous copies: the matrices (dynamics block,
+// Hessian block, the factor of the next stage) by one bulk copy per QP (TMA, cp.async.bulk), issued by lane 0 of the group
+// and completed on the warp's mbarrier; the "images" of the contiguous vector ranges of the three records by 16-byte copies
+// (cp.async) by the lanes of the group, completed by a wait on the lane's copies and a warp barrier.  The arithmetic then runs
+// on shared memory and registers only, results leave through plain stores.  The matrices come from the
 // kernel-side QP record (FastArgs::qpk, written by the repack pass): odd leading dimension (row and column accesses of a
 // group both bank-conflict free), Hessian stored as a full symmetric matrix; the factorisation takes the dynamics block
 // from the caller's record (even leading dimension n: its broadcast operand is read with 128-bit loads).
@@ -27,10 +28,11 @@
 // warp and contraction lengths that are multiples of four the level-3 parts of the factorisation run on the FP64 tensor cores
 // (fk_dmma: mma.m8n8k4), otherwise on register tiles.
 //
-// The file is written against a few warp primitives supplied by the including translation unit (FK_DEV, fk_lane,
-// fk_sync, fk_shfl_xor, fk_any, fk_bulk, fk_dmma, fk_atomic_add / _cas, fk_ld_volatile, fk_threadfence, fk_mbar_*, fk_fence_async, fk_ldg, fk_rsqrt, fk_atomic_inc): the CUDA
-// instantiation is cuipm_fast.cu; oracle/fast_emul.cpp instantiates the same body on a host emulation of a warp for the
-// CPU test-suite.
+// The file is written against a few warp primitives supplied by the including translation unit (FK_DEV, fk_lane, fk_sync,
+// fk_shfl_xor / _i, fk_any, fk_cp16, fk_cp_wait, fk_bulk, fk_mbar_t, fk_mbar_init / _arrive_tx / _wait, fk_fence_async /
+// _global, fk_ldg, fk_double2, fk_ld2, fk_dmma, fk_rsqrt, fk_atomic_inc / _add / _cas, fk_ld_volatile, fk_st_volatile,
+// fk_threadfence, fk_nanosleep): the CUDA instantiation is cuipm_fast.cu; oracle/fast_emul.cpp instantiates the same body on a
+// host emulation of a warp for the CPU test-suite.
 #ifndef CUIPM_FAST_CORE_H_
 #define CUIPM_FAST_CORE_H_
 
@@ -54,39 +56,11 @@
     _Pragma("unroll 1") for (int i_ = inv[jj], i = i_ >= 0 ? i_ : 0, e_ = i_ >= 0 ? i_ + 1 : (i_ == -2 ? nb : 0); i < e_; i++) \
         if (i_ >= 0 || rev[i] == (jj))
 
-// The short loops of a lane over its elements of a vector (run-time trip counts of 1..4) are kept as loops: the compiler's
-// unroll-by-four with a remainder chain executes more instructions than the loop it replaces at these trip counts, and
-// multiplies the instruction footprint of the sweeps (on the headline shape the SASS shrinks from 574 to 337 KB).
-#define FK_PRAGMA_(x) _Pragma(#x)
-#define FK_PRAGMA(x) FK_PRAGMA_(x)
-#ifndef FK_VLOOP_N
-#define FK_VLOOP_N 1
-#endif
-#define FK_VLOOP FK_PRAGMA(unroll FK_VLOOP_N)
-// the loops over the 8-column tiles of a stage: unrolled (row slots above a tile vanish at compile time) or kept as loops
-#ifndef FK_TILE_N
-#define FK_TILE_LOOP _Pragma("unroll")
-#else
-#define FK_TILE_LOOP FK_PRAGMA(unroll FK_TILE_N)
-#endif
-// (the same for the tile loop of the Gram product / panel factorisation alone)
-#ifndef FK_TILE2_N
-#define FK_TILE_LOOP2 FK_TILE_LOOP
-#else
-#define FK_TILE_LOOP2 FK_PRAGMA(unroll FK_TILE2_N)
-#endif
-#ifndef FK_U_DOT
-#define FK_U_DOT 4
-#endif
-#ifndef FK_U_TRMM
-#define FK_U_TRMM 4
-#endif
-#ifndef FK_U_SYRK
-#define FK_U_SYRK 3
-#endif
-#ifndef FK_U_UPD
-#define FK_U_UPD 2
-#endif
+// Unrolling: the short loops of a lane over its elements of a vector (run-time trip counts of 1..4) are kept as loops
+// ("unroll 1"): the compiler's unroll-by-four with a remainder chain executes more instructions than the loop it replaces at
+// these trip counts, and multiplies the instruction footprint of the sweeps (on the headline shape the SASS shrinks from 574
+// to 337 KB).  The loops over the 8-column tiles of a stage are unrolled in full (row slots above a tile vanish at compile
+// time); the inner loops of the dot products, TRMM, SYRK and the left-looking update are unrolled by 4, 4, 3 and 2.
 
 namespace cuipm {
 namespace fastk {
@@ -133,8 +107,7 @@ struct Ker
     static constexpr int SZA = (LDK * NX + 1) & ~1;       // dynamics block [B'; A'] (-> A Lxx in place in the factorisation, leading dimension n there)
     static constexpr int SZL = LDW * NM;                  // L_{k+1} -> L_k (factorisation); Hessian / L_{k+1} (other sweeps)
     static constexpr int SZU = (NM * NU + 1) & ~1;        // first nu columns of L_k (substitutions), leading dimension n
-    static constexpr int SZD = 0;                         // (the diagonal blocks of the factorisation are published in the vector pool)
-    static constexpr int MATS = SZA + SZL + SZU + SZD;
+    static constexpr int MATS = SZA + SZL + SZU;
 
     // FP64 tensor-core tiles (mma.m8n8k4) for the level-3 parts of the factorisation: one QP per warp only (the fragments span
     // the 32 lanes), contraction lengths that are multiples of four
@@ -157,17 +130,14 @@ struct Ker
     const FastArgs &A;
     double *smem0;             // shared memory of the groups of the warp (after the index maps)
     const int *IDX;            // index maps (idxb, idxs_rev), shared by the groups: entry e = (idxb | idxs_rev | its inverse) at IDX + 4*e*nbe (FastArgs::nmaps entries)
-    fk_mbar_t *bars;           // [0]: vector images, [1]: matrices, [2..5]: ring of the mu_aff reduction
-    int li, gq, q0;            // lane within the group, group within the warp, first QP of the warp
-    double *MA, *ML, *LU, *DD, *V;
+    fk_mbar_t *bar;            // completes the bulk copies of the matrices (the vector images complete through wait_vec)
+    int li, gq;                // lane within the group, group within the warp
+    double *MA, *ML, *LU, *V;
     const double *qp, *qk;     // this group's QP record: the caller's, the kernel-side one
     double *sol, *wk;
     bool act;                  // this group's QP is being solved: global stores enabled
-    const double *rbase[4];    // records of the warp's first QP: kernel-side QP record, solution, work, caller's QP record (warp-uniform)
-    size_t rstep[4];           // record strides
-    int nvalid;                // QPs of this warp that exist (the others re-read the last one)
-    unsigned ph0, ph1, phm;    // phase parities of the barriers (phm: one bit per slot of the mu_aff ring); they live as long as the barriers
-    unsigned tx0, tx1;         // bytes announced to them in the phase being filled
+    unsigned ph;               // phase parity of the barrier; it lives as long as the barrier
+    unsigned tx;               // bytes of matrix copies issued and not yet announced to the barrier
     double nc_mask_inv;
 
     struct View { const double *q; const double *k; double *s; double *w; const int *ip; unsigned kk; };
@@ -177,7 +147,6 @@ struct Ker
         const int lane = fk_lane();
         li = lane % G;
         gq = lane / G;
-        q0 = 0;
         // the index maps are the same for every QP (and, checked on the host, for every interior stage): one copy per warp
         int *idx = reinterpret_cast<int *>(smem);
         for (int e = 0; e < a.nmaps; e++)
@@ -206,17 +175,13 @@ struct Ker
         IDX = idx;
         smem += 2 * a.nmaps * a.nbe;
         smem0 = smem;
-        bars = b;
+        bar = b;
         double *S = smem + (size_t) gq * a.gstride;
-        MA = S; ML = MA + SZA; LU = ML + SZL; DD = LU + SZU; V = DD + SZD;
+        MA = S; ML = MA + SZA; LU = ML + SZL; V = LU + SZU;
         qp = nullptr; qk = nullptr; sol = nullptr; wk = nullptr; act = false;
-        ph0 = ph1 = phm = 0; tx0 = tx1 = 0;
+        ph = 0; tx = 0;
         nc_mask_inv = 0.0;
-        rbase[0] = rbase[1] = rbase[2] = rbase[3] = nullptr;
-        rstep[0] = a.qpk_stride; rstep[1] = a.sol_stride; rstep[2] = a.work_stride; rstep[3] = a.qp_stride;
-        nvalid = 0;
-        if (lane == 0)
-            for (int i = 0; i < 6; i++) fk_mbar_init(bars + i, 1);
+        if (lane == 0) fk_mbar_init(bar, 1);
         fk_fence_async();
         fk_sync();
     }
@@ -224,10 +189,6 @@ struct Ker
     // solves QPs first_qp .. first_qp + QPW - 1 (those that exist), one per group
     FK_DEV void run(int first_qp)
     {
-        q0 = first_qp;
-        rbase[0] = A.qpk + (size_t) first_qp * A.qpk_stride; rbase[1] = A.sol + (size_t) first_qp * A.sol_stride; rbase[2] = A.work + (size_t) first_qp * A.work_stride;
-        rbase[3] = A.qp + (size_t) first_qp * A.qp_stride;
-        nvalid = A.nbatch - first_qp < QPW ? A.nbatch - first_qp : QPW;
         int q = first_qp + gq;
         const bool valid = q < A.nbatch;
         if (!valid) q = A.nbatch - 1;
@@ -286,24 +247,20 @@ struct Ker
         return r;
     }
 
-    // ---- staging: bulk asynchronous copies with warp-uniform operands ---------------------------------------------------
-    // One contiguous range of `nd` doubles (even) per QP of the warp, from record REC (0 kernel-side QP record, 1 solution,
-    // 2 work, 3 the caller's QP record) at record offset `off`, to offset `soff` of each group's shared memory; BAR: 0 vector
-    // images, 1 matrices.
-    // Lane 0 issues the copies (operands depend on the warp only); every lane keeps the byte count.
-    // pf = +1 / -1: the same range of the next / previous interior stage is prefetched into L2 (the sweep gets there next)
-    template <int REC, int BAR>
-    FK_DEV void bulk(int soff, size_t off, int nd, int pf = 0)
+    // ---- staging ---------------------------------------------------------------------------------------------------------
+    // Matrices: one contiguous range of `nd` doubles (even) of this group's record REC (0 kernel-side QP record, 1 solution,
+    // 2 work, 3 the caller's QP record) at record offset `off`, to offset `soff` of the group's shared memory, as one bulk
+    // asynchronous copy completed on the barrier.  Lane 0 of every group issues the copy of its QP (the compiler serialises the
+    // 32/G different operand sets); every lane keeps the byte count of the warp.
+    template <int REC>
+    FK_DEV void bulk(int soff, size_t off, int nd)
     {
-        // lane 0 of every group issues the copy of its QP (the compiler serialises the 32/G different operand sets)
         if (li == 0)
         {
-            fk_bulk(smem0 + (size_t) gq * A.gstride + soff, (REC == 0 ? qk : (REC == 1 ? sol : (REC == 2 ? wk : qp))) + off, (unsigned) nd * 8u, bars + BAR);
+            fk_bulk(smem0 + (size_t) gq * A.gstride + soff, (REC == 0 ? qk : (REC == 1 ? sol : (REC == 2 ? wk : qp))) + off, (unsigned) nd * 8u, bar);
             FK_COUNT_STAGED((unsigned) nd * 8u);
         }
-        (void) pf;
-        if (BAR == 0) tx0 += (unsigned) (QPW * nd) * 8u;
-        else tx1 += (unsigned) (QPW * nd) * 8u;
+        tx += (unsigned) (QPW * nd) * 8u;
     }
     // Vector images: contiguous range of `nd` doubles (even) of this group's record REC at record offset `off` -> dst (shared
     // memory of the group), as 16-byte asynchronous copies by the lanes of the group (LDGSTS: all groups of the warp copy at
@@ -313,7 +270,7 @@ struct Ker
     FK_DEV void vcopy(double *dst, size_t off, int nd)
     {
         const double *src = (REC == 0 ? qk : (REC == 1 ? sol : (REC == 2 ? wk : qp))) + off;
-FK_VLOOP
+#pragma unroll 1
         for (int e = 2 * li; e < nd; e += 2 * G)
         {
             fk_cp16(dst + e, src + e);
@@ -325,18 +282,17 @@ FK_VLOOP
     // the copies of this stage have been issued: announce their bytes
     FK_DEV void stage_arm()
     {
-        if (fk_lane() == 0) fk_mbar_arrive_tx(bars + 1, tx1);
-        tx1 = 0;
+        if (fk_lane() == 0) fk_mbar_arrive_tx(bar, tx);
+        tx = 0;
     }
-    FK_DEV void stage_arm_vec() {}
     // matrix copies announced separately (a second batch inside a stage, requests for the next stage)
     FK_DEV void stage_arm_mat()
     {
-        if (fk_lane() == 0) fk_mbar_arrive_tx(bars + 1, tx1);
-        tx1 = 0;
+        if (fk_lane() == 0) fk_mbar_arrive_tx(bar, tx);
+        tx = 0;
     }
     FK_DEV void wait_vec() { FK_PROF_T0(); fk_cp_wait(); fk_sync(); FK_PROF_ADD(5); }      // own copies landed, then everybody's
-    FK_DEV void wait_mat() { FK_PROF_T0(); fk_mbar_wait(bars + 1, ph1); ph1 ^= 1u; FK_PROF_ADD(6); }
+    FK_DEV void wait_mat() { FK_PROF_T0(); fk_mbar_wait(bar, ph); ph ^= 1u; FK_PROF_ADD(6); }
     FK_DEV int voff(const double *p) const { return (int) (p - (smem0 + (size_t) gq * A.gstride)); }
 
     // out[i] = 1 / t[i], i < nc, over the lanes of the group; four reciprocals per lane are in flight at once (a double
@@ -368,7 +324,7 @@ FK_VLOOP
 #pragma unroll
         for (int m = 0; m < RP; m++) o2[m] = 0.0;
         int j = 0;
-FK_PRAGMA(unroll FK_U_DOT)
+#pragma unroll 4
         for (; j + 1 < nc; j += 2)
         {
             const fk_double2 xx = fk_ld2(x + j);
@@ -405,7 +361,7 @@ FK_PRAGMA(unroll FK_U_DOT)
 #pragma unroll
         for (int m = 0; m < CP; m++) { out[m] = 0.0; o2[m] = 0.0; }
         int i = 0;
-FK_PRAGMA(unroll FK_U_DOT)
+#pragma unroll 4
         for (; i + 1 < nr; i += 2)
         {
             const fk_double2 ww = fk_ld2(w + i);
@@ -440,8 +396,8 @@ FK_PRAGMA(unroll FK_U_DOT)
         const StageDesc &s = sdr(k);
         const unsigned kk = (k >= 1 && k < A.N) ? (unsigned) (k - 1) : 0u;
         const int kind = k == 0 ? 0 : (k == A.N ? 2 : 1);
-        if (s.nx1 > 0) bulk<0, 1>(voff(MA), (size_t) A.kq[kind] + (size_t) kk * A.kqs, evn(LDK * s.nx1));
-        bulk<0, 1>(voff(ML), (size_t) A.kq[kind] + (size_t) kk * A.kqs + A.kH[kind], evn(LDK * s.n));
+        if (s.nx1 > 0) bulk<0>(voff(MA), (size_t) A.kq[kind] + (size_t) kk * A.kqs, evn(LDK * s.nx1));
+        bulk<0>(voff(ML), (size_t) A.kq[kind] + (size_t) kk * A.kqs + A.kH[kind], evn(LDK * s.n));
         stage_arm_mat();
     }
 
@@ -495,7 +451,7 @@ FK_PRAGMA(unroll FK_U_DOT)
                 fl |= (a != a);
             }
         }
-FK_VLOOP
+#pragma unroll 1
         for (int j = li; j < 2 * ns; j += G)
         {
             double r = qZ[j] * du[n + j] + rg[n + j] - (mask_dl ? mul_rn(dl[2 * nb + j], msk[2 * nb + j]) : dl[2 * nb + j]);
@@ -525,7 +481,6 @@ FK_VLOOP
         double *SOL = V, *STP = SOL + (A.nve + NXe + 2 * A.nce), *SOLN = STP + (A.nve + NXe + 2 * A.nce), *STPN = SOLN + NMe;
         double *QV = STPN + NMe, *tmp0 = QV + (NXe + NMe + 2 * A.nce + 2 * A.ns2e), *tmp1 = tmp0 + A.nbe, *g_ = tmp1 + A.nbe, *pim = g_ + A.nve;
         double *x1 = pim + NXe, *AF = x1 + NXe;
-        const int pf = (KIND == 1 && k + 1 < A.N) ? 1 : 0;
         stage_begin();
         vcopy<1>(SOL, (size_t) v.kk * A.ss + sd.sol.ux, solN);
         if (update) vcopy<2>(STP, (size_t) v.kk * A.ws + sd.step.ux, stpN);
@@ -541,7 +496,6 @@ FK_VLOOP
             vcopy<1>(SOLN, (size_t) v1.kk * A.ss + s1.sol.ux, n1e);
             if (update) vcopy<2>(STPN, (size_t) v1.kk * A.ws + s1.step.ux, n1e);
         }
-        stage_arm_vec();
         if (KIND == 0) res_issue_mat(k);        // the matrices of every later stage were requested by the stage before it
         wait_vec();
         double *ux = SOL, *pi = SOL + (sd.sol.pi - sd.sol.ux), *lam = SOL + (sd.sol.lam - sd.sol.ux), *t = SOL + (sd.sol.t - sd.sol.ux);
@@ -552,14 +506,14 @@ FK_VLOOP
         if (update)
         {
             double *gu = v.s + sd.sol.ux, *gp = v.s + sd.sol.pi;
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < n + 2 * ns; i += G)
             {
                 const double x = ux[i] + alpha_u * du[i];
                 ux[i] = x;
                 st(gu + i, x);
             }
-FK_VLOOP
+#pragma unroll 1
             for (int j = li; j < nx1; j += G)
             {
                 const double p = pi[j] + alpha_u * dp[j];
@@ -567,12 +521,12 @@ FK_VLOOP
                 st(gp + j, p);
             }
         }
-FK_VLOOP
+#pragma unroll 1
         for (int j = li; j < nx1; j += G) x1[j] = update ? SOLN[nu1 + j] + alpha_u * STPN[nu1 + j] : SOLN[nu1 + j];
         {
             double *gl = v.s + sd.sol.lam, *gt = v.s + sd.sol.t;
             double *bl = wk + A.w_bkp + (sd.sol.lam + v.kk * A.ss), *bt = wk + A.w_bkp + (sd.sol.t + v.kk * A.ss);
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < nc; i += G)
             {
                 double l = lam[i], tt = t[i];
@@ -599,7 +553,7 @@ FK_VLOOP
             }
         }
         fk_sync();
-FK_VLOOP
+#pragma unroll 1
         for (int i = li; i < nb; i += G) tmp0[i] = lam[nb + i] - lam[i];
         wait_mat();
         fk_sync();
@@ -657,7 +611,7 @@ FK_VLOOP
         else
             fk_sync();
         // ---- box scatter, slack rows
-FK_VLOOP
+#pragma unroll 1
         for (int i = li; i < nb; i += G)
         {
             const int ix = idxb[i];
@@ -666,7 +620,7 @@ FK_VLOOP
         }
         if (ns > 0)
         {
-FK_VLOOP
+#pragma unroll 1
             for (int j = li; j < 2 * ns; j += G)
             {
                 const double sj = ux[n + j], zz = qz[j];
@@ -684,7 +638,7 @@ FK_VLOOP
         // ---- res_d, res_m
         {
             double *od = v.w + sd.res.d, *om = v.w + sd.res.m, *obk = v.w + sd.w_rmb;
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < nc; i += G)
             {
                 const double dv = qd[i];
@@ -719,7 +673,7 @@ FK_VLOOP
                 R.f3 |= (a != a);
             }
             double *og = v.w + sd.res.g;
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < n + 2 * ns; i += G)
             {
                 const double r = g_[i];
@@ -729,7 +683,7 @@ FK_VLOOP
                 R.f0 |= (a != a);
             }
         }
-FK_VLOOP
+#pragma unroll 1
         for (int j = li; j < nx1; j += G) pim[j] = pi[j];      // pi_k is "pi_{k-1}" of the next stage
         if (nx1 > 0 && (lin_a || lin_f))
         {
@@ -784,7 +738,7 @@ FK_VLOOP
     FK_DEV void cond_slacks(int nb, int ns, const int *rev, const int *inv, const double *Z, int fact, const double *Gam, const double *gam,
                             const double *rgs, double *Zi, double *ds, double *tmp0, double *tmp1) const
     {
-FK_VLOOP
+#pragma unroll 1
         for (int j = li; j < 2 * ns; j += G)
         {
             const int jj = j < ns ? j : j - ns, offc = j < ns ? 0 : nb;
@@ -799,7 +753,7 @@ FK_VLOOP
             ds[j] = d;
         }
         fk_sync();
-FK_VLOOP
+#pragma unroll 1
         for (int i = li; i < nb; i += G)
         {
             const int j = rev[i];
@@ -941,13 +895,12 @@ FK_VLOOP
         vcopy<2>((smem0 + (size_t) gq * A.gstride + oRES), (size_t) kk * A.ws + s.res.g, (int) (s.res.m - s.res.g) + evn(s.nc));
         vcopy<1>((smem0 + (size_t) gq * A.gstride + oLT), (size_t) kk * A.ss + s.sol.lam, (int) (s.sol.t - s.sol.lam) + evn(s.nc));
         if (s.ns > 0) vcopy<0>((smem0 + (size_t) gq * A.gstride + oZQ), (size_t) A.kq[kind] + (size_t) kk * A.kqs + A.kV[kind] + (s.q_Z - s.q_b), evn(2 * s.ns));
-        stage_arm_vec();
     }
     FK_DEV void fact_issue_mat(int k)
     {
         const StageDesc &s = sdr(k);
         const unsigned kk = (k >= 1 && k < A.N) ? (unsigned) (k - 1) : 0u;
-        if (s.nx1 > 0) bulk<3, 1>(voff(MA), (size_t) kk * A.qs + s.q_BAt, evn(s.n * s.nx1));      // the caller's block: leading dimension n
+        if (s.nx1 > 0) bulk<3>(voff(MA), (size_t) kk * A.qs + s.q_BAt, evn(s.n * s.nx1));      // the caller's block: leading dimension n
         stage_arm_mat();
     }
 
@@ -992,7 +945,7 @@ FK_VLOOP
             // Gamma, gamma (COMPUTE_GAMMA_GAMMA_QP, x_core_qp_ipm_aux.c:38-86)
             const double t_min_inv = A.o.t_min > 0 ? 1.0 / A.o.t_min : 1e30;
             recip_vec(gt, Gam, nc);                  // same lane, same index below: no barrier needed
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < nc; i += G)
             {
                 const double l = gl[i], tt = gt[i], ti = Gam[i];
@@ -1002,7 +955,7 @@ FK_VLOOP
                     Gam[i] = ti * l;
                 gam[i] = ti * (rm[i] - l * rd[i]);
             }
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < n; i += G) dadd[i] = A.o.reg_prim;
         }
         fk_sync();
@@ -1010,7 +963,7 @@ FK_VLOOP
         {
             cond_slacks(nb, ns, rev, inv, ZQ, 1, Gam, gam, rowv + n, Zi, ds, tmp0, tmp1);
             fk_sync();
-FK_VLOOP
+#pragma unroll 1
             for (int j = li; j < 2 * ns; j += G)
             {
                 st(v.w + sd.w_Zsi + j, Zi[j]);
@@ -1019,7 +972,7 @@ FK_VLOOP
         }
         else
         {
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < nb; i += G)
             {
                 tmp0[i] = Gam[i] + Gam[nb + i];
@@ -1027,7 +980,7 @@ FK_VLOOP
             }
             fk_sync();
         }
-FK_VLOOP
+#pragma unroll 1
         for (int i = li; i < nb; i += G)
         {
             const int ix = idxb[i];
@@ -1059,7 +1012,7 @@ FK_VLOOP
                     if (li + G * m < nx1) st(Pb + li + G * m, tt_[m]);
             }
             fk_sync();
-FK_VLOOP
+#pragma unroll 1
             for (int j = li; j < nx1; j += G) alb[j] += lprev[j];
         }
         // the vector images are dead from here on (gradient and diagonal additions are in registers / in their own arrays):
@@ -1104,7 +1057,7 @@ FK_VLOOP
                 }
             }
             else
-FK_TILE_LOOP
+#pragma unroll
             for (int jt = 0; jt < nx1; jt += 8)
             {
                 const int w = nx1 - jt < 8 ? nx1 - jt : 8;
@@ -1130,7 +1083,7 @@ FK_TILE_LOOP
                         for (int m = 0; m < RP; m++) acc[m][q] += a[m] * l;
                     }
                 }
-FK_PRAGMA(unroll FK_U_TRMM)
+#pragma unroll 4
                 for (int c = jt + 8; c < nx1; c++)
                 {
                     double a[RPM > 0 ? RPM : 1];
@@ -1162,7 +1115,7 @@ FK_PRAGMA(unroll FK_U_TRMM)
         // ---- column tiles: SYRK + left-looking Cholesky, rows r >= jt; gradient h = g + AL alb in the first tile
         const double *Hk = v.k + A.kH[KIND];
         double *Lg = v.w + sd.w_L, *lrow = v.w + sd.w_lrow;
-FK_TILE_LOOP2
+#pragma unroll
         for (int jt = 0; jt < n; jt += 8)
         {
             const int w = n - jt < 8 ? n - jt : 8;
@@ -1252,7 +1205,7 @@ FK_TILE_LOOP2
             else {
             if (nx1 > 0)
             {
-FK_PRAGMA(unroll FK_U_SYRK)
+#pragma unroll 3
                 for (int c = 0; c < nx1; c++)
                 {
                     double a[RPM > 0 ? RPM : 1], b[8];
@@ -1282,7 +1235,7 @@ FK_PRAGMA(unroll FK_U_SYRK)
                 stage_begin();
                 fact_issue_mat(k - 1);
             }
-FK_PRAGMA(unroll FK_U_UPD)
+#pragma unroll 2
             for (int c = 0; c < jt; c++)
             {
                 double a[RPM > 0 ? RPM : 1], b[8];
@@ -1323,9 +1276,9 @@ FK_PRAGMA(unroll FK_U_UPD)
         }
         {
             double *li_ = v.w + sd.w_Linv;
-FK_VLOOP
+#pragma unroll 1
             for (int j = li; j < n; j += G) st(li_ + j, Linv[j]);
-FK_VLOOP
+#pragma unroll 1
             for (int j = li; j < nx; j += G) lprev[j] = lvec[nu + j];
         }
     }
@@ -1335,7 +1288,7 @@ FK_VLOOP
         // the factor is built in ML; its strict upper triangle must read as zero (the triangular products of the sweep run
         // over full rows / columns), and the other sweeps leave the Hessian there
         fk_sync();
-FK_VLOOP
+#pragma unroll 1
         for (int e = li; e < SZL; e += G) ML[e] = 0.0;
         fk_fence_async_global();        // the records this sweep reads with bulk copies were written with plain stores by the sweeps before
 
@@ -1367,7 +1320,6 @@ FK_VLOOP
         double *QM = STL + 2 * A.nce, *Gam = QM + (A.nce + A.ns2e), *gam = Gam + A.nce, *tmp0 = gam + A.nce, *tmp1 = tmp0 + A.nbe;
         double *ds = tmp1 + A.nbe, *xprev = ds + A.ns2e, *tmpx = xprev + NXe;
         const bool so = act && stw;
-        const int pf = (KIND == 1 && k > 1) ? -1 : 0;
         stage_begin();
         vcopy<2>(RES, (size_t) v.kk * A.ws + sd.res.g, resN);
         vcopy<1>(LT, (size_t) v.kk * A.ss + sd.sol.lam, ltN);
@@ -1375,8 +1327,8 @@ FK_VLOOP
         vcopy<2>(RMB, (size_t) v.kk * A.ws + sd.w_rmb, evn(nc));
         vcopy<2>(STL, (size_t) v.kk * A.ws + sd.step.lam, stN);
         vcopy<0>(QM, (size_t) A.kq[KIND] + (size_t) v.kk * A.kqs + A.kV[KIND] + (sd.q_dmask - sd.q_b), qmN);
-        if (nx1 > 0) bulk<0, 1>(voff(MA), (size_t) A.kq[KIND] + (size_t) v.kk * A.kqs, evn(LDK * nx1), pf);
-        if (nsolve > 0) bulk<2, 1>(voff(LU), (size_t) v.kk * A.ws + sd.w_L, evn(n * nsolve), pf);
+        if (nx1 > 0) bulk<0>(voff(MA), (size_t) A.kq[KIND] + (size_t) v.kk * A.kqs, evn(LDK * nx1));
+        if (nsolve > 0) bulk<2>(voff(LU), (size_t) v.kk * A.ws + sd.w_L, evn(n * nsolve));
         stage_arm();
         wait_vec();
         double *vv = RES;
@@ -1387,7 +1339,7 @@ FK_VLOOP
             double *grm = v.w + sd.res.m;
             const double t_min_inv = A.o.t_min > 0 ? 1.0 / A.o.t_min : 1e30;
             recip_vec(gt, Gam, nc);
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < nc; i += G)
             {
                 const double l = gl[i], tt = gt[i], ti = Gam[i];
@@ -1405,19 +1357,19 @@ FK_VLOOP
             cond_slacks(nb, ns, rev, inv, qZ, 0, Gam, gam, vv + n, const_cast<double *>(Zi), ds, tmp0, tmp1);
             fk_sync();
             double *o_ = v.w + sd.step.ux + n;
-FK_VLOOP
+#pragma unroll 1
             for (int j = li; j < 2 * ns; j += G)
                 if (so) o_[j] = ds[j];
         }
         else
         {
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < nb; i += G) tmp1[i] = gam[i] - gam[nb + i];
             fk_sync();
         }
-FK_VLOOP
+#pragma unroll 1
         for (int i = li; i < nb; i += G) vv[idxb[i]] += tmp1[i];
-FK_VLOOP
+#pragma unroll 1
         for (int j = li; j < nx1; j += G) tmpx[j] = xprev[j] + pbs[j];
         wait_mat();
         fk_sync();
@@ -1522,7 +1474,6 @@ FK_VLOOP
         View v1 = v;
         const StageDesc *s1p = &sd;
         if (nx1 > 0) { s1p = &sdr(k + 1); v1 = viewr(k + 1); }
-        const int pf = (KIND == 1 && k + 2 < A.N) ? 1 : 0;
         stage_begin();
         vcopy<2>(RES, (size_t) v.kk * A.ws + sd.res.b, resN);
         vcopy<1>(LT, (size_t) v.kk * A.ss + sd.sol.lam, ltN);
@@ -1533,10 +1484,10 @@ FK_VLOOP
         {
             // p part (gradient vector of stage k+1) / backward value of x_{k+1}
             vcopy<2>(P1, (size_t) v1.kk * A.ws + (after_fact ? s1p->w_lrow : s1p->step.ux), n1e);
-            bulk<0, 1>(voff(MA), (size_t) A.kq[KIND] + (size_t) v.kk * A.kqs, evn(LDK * nx1), pf);
+            bulk<0>(voff(MA), (size_t) A.kq[KIND] + (size_t) v.kk * A.kqs, evn(LDK * nx1));
         }
-        if (nsolve > 0) bulk<2, 1>(voff(LU), (size_t) v.kk * A.ws + sd.w_L, evn(n * nsolve), pf);
-        if (nx1 > 0) bulk<2, 1>(voff(ML), (size_t) v1.kk * A.ws + s1p->w_Lxx, evn((nx1 | 1) * nx1), pf);
+        if (nsolve > 0) bulk<2>(voff(LU), (size_t) v.kk * A.ws + sd.w_L, evn(n * nsolve));
+        if (nx1 > 0) bulk<2>(voff(ML), (size_t) v1.kk * A.ws + s1p->w_Lxx, evn((nx1 | 1) * nx1));
         stage_arm();
         wait_vec();
         const double *bs = RES, *rds = RES + (sd.res.d - sd.res.b), *rms = RES + (sd.res.m - sd.res.b);
@@ -1545,10 +1496,10 @@ FK_VLOOP
         const double *mks = QM;
         {
             const double *src = after_fact ? lrow_ : SUX;
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < nsolve; i += G) vv[i] = -src[i];
             // x part (k>0) was written into vv by the previous stage
-FK_VLOOP
+#pragma unroll 1
             for (int j = li; j < 2 * ns; j += G) dsv[j] = SUX[n + j];
         }
         wait_mat();
@@ -1583,7 +1534,7 @@ FK_VLOOP
         }
         {
             double *o_ = v.w + sd.step.ux, *oa = v.w + sd.ires.g;
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < n; i += G)
             {
                 if (so) o_[i] = vv[i];
@@ -1619,7 +1570,7 @@ FK_VLOOP
         // ---- constraint part of the step at this stage
         {
             recip_vec(ts, tis, nc);
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < nb; i += G)
             {
                 const double a = vv[idxb[i]];
@@ -1630,7 +1581,7 @@ FK_VLOOP
             {
                 fk_sync();
                 const double t_min_inv = A.o.t_min > 0 ? 1.0 / A.o.t_min : 1e30;
-FK_VLOOP
+#pragma unroll 1
                 for (int j = li; j < 2 * ns; j += G)
                 {
                     const int jj = j < ns ? j : j - ns, offc = j < ns ? 0 : nb;
@@ -1646,14 +1597,14 @@ FK_VLOOP
                     dt[2 * nb + j] = d;
                 }
                 fk_sync();
-FK_VLOOP
+#pragma unroll 1
                 for (int i = li; i < 2 * nb; i += G)
                 {
                     const int up = i >= nb, ii = up ? i - nb : i;
                     if (rev[ii] >= 0) dt[i] += dsv[(up ? ns : 0) + rev[ii]];
                 }
                 double *o_ = v.w + sd.step.ux + n, *oa = v.w + sd.ires.g + n;
-FK_VLOOP
+#pragma unroll 1
                 for (int j = li; j < 2 * ns; j += G)
                 {
                     if (so) o_[j] = dsv[j];
@@ -1662,7 +1613,7 @@ FK_VLOOP
             }
             fk_sync();
             double *odl = v.w + sd.step.lam, *odt = v.w + sd.step.t, *oa = v.w + sd.ires.d;
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < nc; i += G)
             {
                 const double l = lam[i], tt = ts[i], ti = tis[i], rdi = rds[i], rmi = rms[i];
@@ -1727,7 +1678,7 @@ FK_VLOOP
         FK_PROF_ADD2(21);      /* pi */
         if (nx1 > 0)
         {
-FK_VLOOP
+#pragma unroll 1
             for (int j = li; j < nx1; j += G) vv[nu1 + j] = x1[j];
         }
     }
@@ -1766,7 +1717,7 @@ FK_VLOOP
             const StageDesc &s = sdr(k);
             const View v = viewr(k);
             const double *l = v.s + s.sol.lam, *t = v.s + s.sol.t, *dl = v.w + s.step.lam, *dt = v.w + s.step.t;
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < s.nc; i += G) acc += fabs((l[i] + alpha * dl[i]) * (t[i] + alpha * dt[i]));
         };
         plain(0);
@@ -1822,11 +1773,11 @@ FK_VLOOP
                 double *l = v.s + s.sol.lam, *t = v.s + s.sol.t, *gux = v.s + s.sol.ux, *gpi = v.s + s.sol.pi;
                 // keep what the caller passed in for the case that this QP is handed back to the generic kernel
                 double *kl = v.w + s.itref.lam, *kt = v.w + s.itref.t, *kp = v.w + s.itref.pi;
-FK_VLOOP
+#pragma unroll 1
                 for (int i = li; i < s.n + 2 * s.ns; i += G) st(gux + i, 0.0);
-FK_VLOOP
+#pragma unroll 1
                 for (int i = li; i < s.nx1; i += G) st(kp + i, gpi[i]);
-FK_VLOOP
+#pragma unroll 1
                 for (int i = li; i < s.nc; i += G)
                 {
                     st(kl + i, l[i]);
@@ -1847,21 +1798,21 @@ FK_VLOOP
             const int *idxb = IDX + 4 * (A.nmaps == 3 ? (k == 0 ? 0 : (k == A.N ? 2 : 1)) : k) * A.nbe, *rev = idxb + nb;
             const double *d = v.q + s.q_d;
             double *gux = v.s + s.sol.ux, *gpi = v.s + s.sol.pi, *gl = v.s + s.sol.lam, *gt = v.s + s.sol.t;
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < s.nx1; i += G) st(gpi + i, 0.0);
             if (A.o.t0_init == 0 || A.o.t0_init == 1)
             {
                 const double l0 = A.o.t0_init == 0 ? sqrt(A.o.mu0) : A.o.mu0, t0 = A.o.t0_init == 0 ? sqrt(A.o.mu0) : 1.0;
-FK_VLOOP
+#pragma unroll 1
                 for (int i = li; i < n + 2 * ns; i += G) st(gux + i, 0.0);
-FK_VLOOP
+#pragma unroll 1
                 for (int i = li; i < nc; i += G) { st(gl + i, l0); st(gt + i, t0); }
                 continue;
             }
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < n + 2 * ns; i += G) ux[i] = 0.0;
             fk_sync();
-FK_VLOOP
+#pragma unroll 1
             for (int j = li; j < 2 * ns; j += G)
             {
                 double tj = ux[n + j] - d[2 * nb + j];
@@ -1873,7 +1824,7 @@ FK_VLOOP
                 tt[2 * nb + j] = tj;
             }
             fk_sync();
-FK_VLOOP
+#pragma unroll 1
             for (int j = li; j < nb; j += G)
             {
                 const int ix = idxb[j];
@@ -1903,9 +1854,9 @@ FK_VLOOP
                 tt[nb + j] = tu;
             }
             fk_sync();
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < n + 2 * ns; i += G) st(gux + i, ux[i]);
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < nc; i += G)
             {
                 st(gt + i, tt[i]);
@@ -1935,7 +1886,7 @@ FK_VLOOP
         const int N = A.N;
         const int SM = CUIPM_STAT_M;
         if (stat && act)
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < SM * (A.o.stat_max + 1); i += G) stat[i] = 0.0;
 
         // constraint mask census (x_ocp_qp_ipm.c:2774-2806)
@@ -1944,7 +1895,7 @@ FK_VLOOP
         {
             const StageDesc &s = sdr(k);
             const double *gm = viewr(k).q + s.q_dmask;
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < s.nc; i += G) cnt += fk_ldg(gm + i) != 0.0;
         }
         const int nc_mask = (int) (gsum((double) cnt) + 0.5);
@@ -1961,7 +1912,7 @@ FK_VLOOP
             const View v = viewr(k);
             double *l = v.s + s.sol.lam;
             const double *gm = v.q + s.q_dmask;
-FK_VLOOP
+#pragma unroll 1
             for (int i = li; i < s.nc; i += G) st(l + i, l[i] * fk_ldg(gm + i));
         }
         fk_sync();
@@ -2317,6 +2268,21 @@ inline int vector_pool_doubles(int NX, int NM, int nce, int nbe, int ns2e, int n
     if (v_fwd > m) m = v_fwd;
     if (v_init > m) m = v_init;
     return m + 8;
+}
+
+// Shared-memory layout of instance <NX, NU, G> for the shape planned in F: sets F.vsize (vector pool) and F.gstride (doubles
+// per QP) and returns the dynamic shared memory of one CTA (one warp) in bytes: the index maps, then the areas of its groups.
+// 32 / G groups share a warp; 64-bit shared loads are served per half-warp: a group stride of 8 (mod 16) doubles puts the
+// consecutive-row accesses of the two groups of a half-warp on disjoint banks.
+template <int NX, int NU, int G>
+inline size_t layout(FastArgs &F)
+{
+    using K = Ker<NX, NU, G>;
+    F.vsize = vector_pool_doubles(NX, NX + NU, F.nce, F.nbe, F.ns2e, F.nve);
+    int gs = K::MATS + F.vsize;
+    while (gs % 16 != 8) gs++;
+    F.gstride = gs;
+    return sizeof(double) * ((size_t) F.gstride * K::QPW + 2 * (size_t) F.nmaps * F.nbe);
 }
 
 }  // namespace fastk

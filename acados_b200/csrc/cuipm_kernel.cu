@@ -2045,9 +2045,8 @@ __global__ void __launch_bounds__(32 * W, (W == 1 ? CUIPM_MINB : (W == 2 ? 8 : 4
 
 }  // namespace
 
-size_t smem_bytes(const ProbDesc &P) { return sizeof(double) * (size_t) P.sm_total; }
-
-int max_warps() { return 4; }
+// dynamic shared memory (bytes) the kernel needs for P
+static size_t smem_bytes(const ProbDesc &P) { return sizeof(double) * (size_t) P.sm_total; }
 
 template <int W, int SNX, int SNU>
 static cudaError_t launch_one(const LaunchArgs &a, size_t smem, cudaStream_t stream)

@@ -26,20 +26,10 @@ static inline void fk_cp_wait() { simt::cp_wait(); }
 typedef simt::MBar fk_mbar_t;
 static inline void fk_mbar_init(fk_mbar_t *b, int count) { simt::mbar_init(b, count); }
 static inline void fk_bulk(double *dst, const double *src, unsigned bytes, fk_mbar_t *b) { simt::bulk_copy(b, dst, src, (int) bytes); }
-static inline void fk_bulk_groups(double *sdst, const double *gsrc, unsigned bytes, fk_mbar_t *b, int n, int gstride, size_t rstep, int nvalid)
-{
-    for (int g = 0; g < n; g++)
-    {
-        fk_bulk(sdst, gsrc, bytes, b);
-        sdst += gstride;
-        if (g + 1 < nvalid) gsrc += rstep;
-    }
-}
 static inline void fk_mbar_arrive_tx(fk_mbar_t *b, unsigned bytes) { simt::mbar_arrive_tx(b, (int) bytes); }
 static inline void fk_mbar_wait(fk_mbar_t *b, unsigned parity) { simt::mbar_wait(b, (int) parity); }
 static inline void fk_fence_async() {}
 static inline void fk_fence_async_global() {}
-static inline void fk_prefetch_l2(const double *, unsigned) {}
 static inline double fk_ldg(const double *p) { return *p; }
 struct fk_double2 { double x, y; };
 static inline fk_double2 fk_ld2(const double *p)
@@ -72,11 +62,7 @@ template <int NX, int NU, int G>
 int run(cuipm::FastArgs F, int order)
 {
     using K = cuipm::fastk::Ker<NX, NU, G>;
-    F.vsize = cuipm::fastk::vector_pool_doubles(NX, NX + NU, F.nce, F.nbe, F.ns2e, F.nve);
-    int gs = K::MATS + F.vsize;
-    while (gs % 16 != 8) gs++;
-    F.gstride = gs;
-    std::vector<double> smem((size_t) gs * K::QPW + 2 * (size_t) F.nmaps * F.nbe + 64);
+    std::vector<double> smem(cuipm::fastk::layout<NX, NU, G>(F) / sizeof(double) + 64);
     // 16-byte aligned base
     double *base = smem.data();
     while ((size_t) base & 15) base++;
@@ -87,9 +73,9 @@ int run(cuipm::FastArgs F, int order)
     for (int w = 0; w < nwarp; w++)
     {
         for (double &x : smem) x = std::nan("");      // uninitialised shared memory
-        simt::MBar bars[6];
+        simt::MBar bar;
         simt::run_warp([&]() {
-            K k(F, base, bars);
+            K k(F, base, &bar);
             if (g_rr) k.rr_first(w * K::QPW);
             else k.run(w * K::QPW);
         }, order);
@@ -100,9 +86,9 @@ int run(cuipm::FastArgs F, int order)
         for (int w = 0; w < (nwarp < 3 ? nwarp : 3); w++)
         {
             for (double &x : smem) x = std::nan("");
-            simt::MBar bars[6];
+            simt::MBar bar;
             simt::run_warp([&]() {
-                K k(F, base, bars);
+                K k(F, base, &bar);
                 k.rr_loop();
             }, order);
         }
