@@ -28,9 +28,10 @@ struct StageDesc
     unsigned q_stage, q_stage_bytes;      // this stage's sub-record inside the QP record (16-byte multiple)
     unsigned w_fac, w_fac_bytes;          // factor part of the work record (L, Linv, lrow, Pb, Zs_inv)
     unsigned w_vec, w_vec_bytes;          // vector part of the work record
-    unsigned w_Lxx;                       // work record: copy of the state block Lxx of L (nx x nx, leading dimension nx|1, zero above the
-                                          // diagonal) kept by the throughput kernel for its forward sweeps (odd leading dimension: row and
-                                          // column accesses both bank-conflict free); sizeof(StageDesc) stays a multiple of 8
+    unsigned w_Lxx;                       // work record: copy of the state block Lxx of L kept by the throughput kernel for its forward
+                                          // sweeps, room for nx x nx with leading dimension nx|1: its packed lower triangle (nx (nx + 1) / 2,
+                                          // column by column, fastk::tri) where FastArgs::packed, else the full block with leading dimension
+                                          // nx|1 (zero above the diagonal); sizeof(StageDesc) stays a multiple of 8
 };
 static_assert(sizeof(StageDesc) % 8 == 0, "StageDesc must be a multiple of 8 bytes");
 
@@ -87,11 +88,13 @@ struct FastArgs
     size_t qp_stride, sol_stride, work_stride;
     StageDesc s0, s1, sN;
     // kernel-side QP records (written by the repack pass from the caller's records): per stage [BAt with leading dimension
-    // ld | RSQ as a full symmetric matrix with leading dimension ld | the vectors b, rq, d, d_mask, Z, z as in the caller's
-    // record]; kq = start of the stage (stages 0, 1, N), kqs = stride of the interior stages, kH / kV = offsets of the
-    // symmetric Hessian / the vector part inside the stage
+    // ld | RSQ: its lower triangle packed column by column (n (n + 1) / 2, fastk::tri) if packed, else the full symmetric
+    // matrix with leading dimension ld | the vectors b, rq, d, d_mask, Z, z as in the caller's record]; kq = start of the
+    // stage (stages 0, 1, N), kqs = stride of the interior stages, kH / kV = offsets of the Hessian / the vector part inside
+    // the stage
     unsigned kq[3], kH[3], kV[3], kqs;
     int ld;
+    int packed;                    // fast_packed(nx, nu) of the interior stages: Hessian and w_Lxx hold packed triangles
     size_t qpk_stride;
     const double *qpk;
     const int *ipool;
@@ -111,6 +114,13 @@ struct FastArgs
     int *rr_ctr;
     cuipm_opts o;
 };
+
+// Whether the throughput kernel stages the Hessian and the state block of the next stage's factor as packed lower triangles
+// (half the bytes of the full blocks) for interior stages (nx, nu).  Stage blocks of up to 32 rows run several QPs per warp and
+// the kernel's time follows the bytes it stages.  Larger blocks (the legged shape) run one QP per warp, a few warps per SM,
+// and are bound by the latency of the arithmetic: there the index arithmetic and the bank conflicts of the packed reads cost
+// more than the halved copies save, so they keep the full blocks.
+constexpr bool fast_packed(int nx, int nu) { return nx + nu <= 32; }
 
 #define CUIPM_RR_RINGS 8
 #define CUIPM_RR_CTR 32

@@ -139,8 +139,9 @@ __global__ void __launch_bounds__(32, MINB) cuipm_fast_kernel(const __grid_const
 #endif
 }
 
-// caller's QP records -> kernel-side records: dynamics block with leading dimension ld, Hessian as a full symmetric matrix
-// with leading dimension ld (lower triangle mirrored), vector part verbatim.  One CTA per QP, coalesced writes.
+// caller's QP records -> kernel-side records: dynamics block with leading dimension ld, the lower triangle of the Hessian
+// packed column by column (fastk::tri; only the lower triangle is read) or, unless A.packed, the full symmetric matrix with
+// leading dimension ld (lower triangle mirrored), vector part verbatim.  One CTA per QP, coalesced writes.
 __global__ void __launch_bounds__(256) cuipm_repack_kernel(const FastArgs A, const StageDesc *__restrict__ sd)
 {
     const int N = A.N, ld = A.ld;
@@ -163,7 +164,12 @@ __global__ void __launch_bounds__(256) cuipm_repack_kernel(const FastArgs A, con
             for (int e = threadIdx.x; e < n * n; e += blockDim.x)
             {
                 const int j = e / n, i = e - j * n;
-                H[i + ld * j] = i >= j ? qp[d.q_RSQ + e] : qp[d.q_RSQ + j + n * i];
+                if (A.packed)
+                {
+                    if (i >= j) H[fastk::tri(n, i, j)] = qp[d.q_RSQ + e];
+                }
+                else
+                    H[i + ld * j] = i >= j ? qp[d.q_RSQ + e] : qp[d.q_RSQ + j + n * i];
             }
             const int nv = (int) (d.q_stage + d.q_stage_bytes / 8u - d.q_b);
             for (int e = threadIdx.x; e < nv; e += blockDim.x) o[A.kV[kind] + e] = qp[d.q_b + e];

@@ -7,13 +7,17 @@
 // travels as a vector next to the factorisation (a fused right-looking substitution), so the row slots hold matrix rows only.
 //
 // Data movement: every input of a stage is brought into shared memory by asynchronous copies: the matrices (dynamics block,
-// Hessian block, the factor of the next stage) by one bulk copy per QP (TMA, cp.async.bulk), issued by lane 0 of the group
-// and completed on the warp's mbarrier; the "images" of the contiguous vector ranges of the three records by 16-byte copies
-// (cp.async) by the lanes of the group, completed by a wait on the lane's copies and a warp barrier.  The arithmetic then runs
-// on shared memory and registers only, results leave through plain stores.  The matrices come from the
-// kernel-side QP record (FastArgs::qpk, written by the repack pass): odd leading dimension (row and column accesses of a
-// group both bank-conflict free), Hessian stored as a full symmetric matrix; the factorisation takes the dynamics block
-// from the caller's record (even leading dimension n: its broadcast operand is read with 128-bit loads).
+// Hessian block, the state block of the factor of the next stage) by one bulk copy per QP (TMA, cp.async.bulk), issued by
+// lane 0 of the group and completed on the warp's mbarrier; the "images" of the contiguous vector ranges of the three records
+// by 16-byte copies (cp.async) by the lanes of the group, completed by a wait on the lane's copies and a warp barrier.  The
+// arithmetic then runs on shared memory and registers only, results leave through plain stores.  The dynamics block and the
+// Hessian come from the kernel-side QP record (FastArgs::qpk, written by the repack pass): the dynamics block with an odd
+// leading dimension (row and column accesses of a group both bank-conflict free), the Hessian as its packed lower triangle
+// (tri: half the bytes of the full symmetric matrix; the products keep the order of summation of the full matrix and give
+// bit-identical results); the factorisation takes the dynamics block from the caller's record
+// (even leading dimension n: its broadcast operand is read with 128-bit loads).  The forward sweeps read the state block Lxx
+// of the next stage's factor from the packed lower triangle the factorisation leaves in the work record (StageDesc::w_Lxx).
+// Stage blocks of more than 32 rows keep both as full matrices with odd leading dimensions (fast_packed, Ker::PACK).
 //
 // Algorithm and work-record layout are those of the generic kernel (cuipm_kernel.cu), which restates HPIPM's
 // d_ocp_qp_ipm_solve (external/hpipm/ocp_qp/x_ocp_qp_ipm.c:2684-3120): the sensitivity kernel and the Riccati getters
@@ -66,6 +70,8 @@ namespace cuipm {
 namespace fastk {
 
 FK_DEV int evn(int n) { return (n + 1) & ~1; }
+// packed lower triangle of an n x n matrix, column by column: offset of element (i, j), i >= j (n (n + 1) / 2 doubles)
+FK_DEV constexpr int tri(int n, int i, int j) { return j * (2 * n - j - 1) / 2 + i; }
 
 // a product rounded before it is used: never contracted into an FMA with the sum it enters (the host build of the emulation
 // has no FMA to contract into)
@@ -101,11 +107,12 @@ struct Ker
     static constexpr int QPW = 32 / G;                    // QPs per warp
     static constexpr int LDK = NM | 1;                     // leading dimension of the kernel-side record (odd: row and column accesses
                                                           // of a group in shared memory are both bank-conflict free)
+    static constexpr bool PACK = fast_packed(NX, NU);     // Hessian and Lxx copy staged as packed triangles (FastArgs::packed)
     static constexpr int LDW = ((NM + 1) / 4) * 4 + 2;    // leading dimension of the factor being built (>= NM, = 2 mod 4: 16-byte aligned columns)
     static constexpr int RPM = (NM + G - 1) / G;          // row slots per lane
     static constexpr int NXe = (NX + 1) & ~1, NMe = (NM + 2) & ~1;
     static constexpr int SZA = (LDK * NX + 1) & ~1;       // dynamics block [B'; A'] (-> A Lxx in place in the factorisation, leading dimension n there)
-    static constexpr int SZL = LDW * NM;                  // L_{k+1} -> L_k (factorisation); Hessian / L_{k+1} (other sweeps)
+    static constexpr int SZL = LDW * NM;                  // L_{k+1} -> L_k (factorisation); Hessian (residual sweep), Lxx_{k+1} (forward sweeps)
     static constexpr int SZU = (NM * NU + 1) & ~1;        // first nu columns of L_k (substitutions), leading dimension n
     static constexpr int MATS = SZA + SZL + SZU;
 
@@ -313,9 +320,39 @@ struct Ker
     }
 
     // ---- small dense helpers on shared memory -----------------------------------------------------------------------
-    // y[i] (+)= sum_j M[i + ld*j] * x[j], j < nc, for the rows i = li, li+G, ... < nr of this lane (row access), x broadcast
-    template <int nr, int nc>
-    FK_DEV void rows_dot(const double *M, int ld, const double *x, double (&out)[RPM > 0 ? RPM : 1]) const
+    // element (i, j) of a matrix: column-major with leading dimension ld (Dense); the staged Hessian of a stage with n rows
+    // (Hess); the staged state block Lxx (n x n, lower triangular) of the next stage's factor (Lxx).  Where PACK, the last two
+    // are packed lower triangles (tri): Hess reads (j, i) above the diagonal, Lxx selects a 0.0 there -- the product with it
+    // is still formed, as with the stored zero of the full block: NaN, Inf and signed zeros come out as from the full matrix.
+    // Lxx loads before it selects (for 0 <= i, j < n, tri(n, i, j) < n (n + 1) / 2 also when i < j): a predicated load made
+    // the compiler spill more registers in the forward sweeps.
+    struct Dense
+    {
+        const double *M;
+        int ld;
+        FK_DEV double operator()(int i, int j) const { return M[i + ld * j]; }
+    };
+    template <int n>
+    struct Hess
+    {
+        const double *P;
+        FK_DEV double operator()(int i, int j) const { return PACK ? P[i >= j ? tri(n, i, j) : tri(n, j, i)] : P[i + LDK * j]; }
+    };
+    template <int n>
+    struct Lxx
+    {
+        const double *P;
+        FK_DEV double operator()(int i, int j) const
+        {
+            if (!PACK) return P[i + (n | 1) * j];
+            const double v = P[tri(n, i, j)];
+            return i >= j ? v : 0.0;
+        }
+    };
+
+    // y[i] (+)= sum_j M(i, j) * x[j], j < nc, for the rows i = li, li+G, ... < nr of this lane (row access), x broadcast
+    template <int nr, int nc, class Mat>
+    FK_DEV void rows_dot(const Mat &M, const double *x, double (&out)[RPM > 0 ? RPM : 1]) const
     {
         constexpr int RP = (nr + G - 1) / G;
 #pragma unroll
@@ -334,8 +371,8 @@ struct Ker
             {
                 const int r = li + G * m;
                 const int rr = r < nr ? r : 0;
-                out[m] += M[rr + ld * j] * x0;
-                o2[m] += M[rr + ld * (j + 1)] * x1;
+                out[m] += M(rr, j) * x0;
+                o2[m] += M(rr, j + 1) * x1;
             }
         }
         if (j < nc)
@@ -346,15 +383,15 @@ struct Ker
             {
                 const int r = li + G * m;
                 const int rr = r < nr ? r : 0;
-                out[m] += M[rr + ld * j] * x0;
+                out[m] += M(rr, j) * x0;
             }
         }
 #pragma unroll
         for (int m = 0; m < RP; m++) out[m] += o2[m];
     }
-    // z[j] = sum_i M[i + ld*j] * w[i], i < nr, for the columns j = li, li+G, ... < nc of this lane (column access), w broadcast
-    template <int nr, int nc>
-    FK_DEV void cols_dot(const double *M, int ld, const double *w, double (&out)[RPM > 0 ? RPM : 1]) const
+    // z[j] = sum_i M(i, j) * w[i], i < nr, for the columns j = li, li+G, ... < nc of this lane (column access), w broadcast
+    template <int nr, int nc, class Mat>
+    FK_DEV void cols_dot(const Mat &M, const double *w, double (&out)[RPM > 0 ? RPM : 1]) const
     {
         constexpr int CP = (nc + G - 1) / G;
         double o2[RPM > 0 ? RPM : 1];
@@ -371,8 +408,8 @@ struct Ker
             {
                 const int c = li + G * m;
                 const int cc = c < nc ? c : 0;
-                out[m] += M[i + ld * cc] * w0;
-                o2[m] += M[i + 1 + ld * cc] * w1;
+                out[m] += M(i, cc) * w0;
+                o2[m] += M(i + 1, cc) * w1;
             }
         }
         if (i < nr)
@@ -383,21 +420,21 @@ struct Ker
             {
                 const int c = li + G * m;
                 const int cc = c < nc ? c : 0;
-                out[m] += M[i + ld * cc] * w0;
+                out[m] += M(i, cc) * w0;
             }
         }
 #pragma unroll
         for (int m = 0; m < CP; m++) out[m] += o2[m];
     }
 
-    // matrices of stage k of the residual sweep: dynamics block and symmetric Hessian of the kernel-side record
+    // matrices of stage k of the residual sweep: dynamics block and Hessian (packed where PACK) of the kernel-side record
     FK_DEV void res_issue_mat(int k)
     {
         const StageDesc &s = sdr(k);
         const unsigned kk = (k >= 1 && k < A.N) ? (unsigned) (k - 1) : 0u;
         const int kind = k == 0 ? 0 : (k == A.N ? 2 : 1);
         if (s.nx1 > 0) bulk<0>(voff(MA), (size_t) A.kq[kind] + (size_t) kk * A.kqs, evn(LDK * s.nx1));
-        bulk<0>(voff(ML), (size_t) A.kq[kind] + (size_t) kk * A.kqs + A.kH[kind], evn(LDK * s.n));
+        bulk<0>(voff(ML), (size_t) A.kq[kind] + (size_t) kk * A.kqs + A.kH[kind], evn(PACK ? s.n * (s.n + 1) / 2 : LDK * s.n));
         stage_arm_mat();
     }
 
@@ -406,7 +443,7 @@ struct Ker
     // UPDATE_VAR_QP fused (x_core_qp_ipm_aux.c:472-582: the iterate first moves by alpha_u along the step, with the
     // step shortening and the t/lam clipping) and the affine complementarity right-hand side of the next
     // iteration (res_m = lam*t - tau_min, backup lam*t; BACKUP_RES_M / COMPUTE_TAU_MIN_QP :672-781).
-    // Staged: dynamics block, symmetric Hessian, the solution and step records of the stage, ux of the next stage, the
+    // Staged: dynamics block, Hessian, the solution and step records of the stage, ux of the next stage, the
     // vector part of the QP record.
     // ---------------------------------------------------------------------------------------------
     struct ResAcc
@@ -422,7 +459,7 @@ struct Ker
     // stationarity rows of the residual of the linear system of one step (dux, dpi_k, dlam: du, dp, dl; dl is masked unless mask_dl;
     // dpi_{k-1}: pm) -> inf-norm mx / NaN flag fl:  ((H dux + rhs_g) - dpi_{k-1} + A dpi_k) + bound multipliers, slack rows
     // Z ds + rhs_g - multipliers; a masked multiplier step is rounded before it is summed (OCP_QP_RES_COMPUTE_LIN).  ML, MA:
-    // Hessian and dynamics block; rg: rhs_g (residual set 0 of the iterate the step was computed at).
+    // staged Hessian (Hess) and dynamics block; rg: rhs_g (residual set 0 of the iterate the step was computed at).
     template <int KIND>
     FK_DEV void lin_rows(const double *du, const double *dp, const double *dl, bool mask_dl, const double *msk, const double *rg,
                          const double *qZ, const int *idxb, const int *rev, const int *inv, int nb, int ns, const double (&pm)[RPM > 0 ? RPM : 1],
@@ -431,8 +468,8 @@ struct Ker
         constexpr int nx = KD<KIND>::nx, nu = KD<KIND>::nu, n = nx + nu, nx1 = KD<KIND>::nx1;
         constexpr int RP = (n + G - 1) / G;
         double hx[RPM > 0 ? RPM : 1], ap[RPM > 0 ? RPM : 1];
-        rows_dot<n, n>(ML, LDK, du, hx);
-        if (nx1 > 0) rows_dot<n, nx1>(MA, LDK, dp, ap);
+        rows_dot<n, n>(Hess<n>{ML}, du, hx);
+        if (nx1 > 0) rows_dot<n, nx1>(Dense{MA, LDK}, dp, ap);
 #pragma unroll
         for (int m = 0; m < RP; m++)
         {
@@ -562,8 +599,8 @@ struct Ker
         // ---- rows of res_g (lane = row), res_b (lane = column)
         {
             double hx[RPM > 0 ? RPM : 1], ap[RPM > 0 ? RPM : 1];
-            rows_dot<n, n>(ML, LDK, ux, hx);
-            if (nx1 > 0) rows_dot<n, nx1>(MA, LDK, pi, ap);
+            rows_dot<n, n>(Hess<n>{ML}, ux, hx);
+            if (nx1 > 0) rows_dot<n, nx1>(Dense{MA, LDK}, pi, ap);
 #pragma unroll
             for (int m = 0; m < RP; m++)
             {
@@ -583,7 +620,7 @@ struct Ker
             if (nx1 > 0)
             {
                 double au[RPM > 0 ? RPM : 1];
-                cols_dot<n, nx1>(MA, LDK, ux, au);
+                cols_dot<n, nx1>(Dense{MA, LDK}, ux, au);
                 double *ob = v.w + sd.res.b;
 #pragma unroll
                 for (int m = 0; m < CP; m++)
@@ -862,14 +899,18 @@ struct Ker
 #pragma unroll
                     for (int q = 0; q < W; q++)
                         if (rr >= q) gr[q * n] = xs[q];
-                    // state block once more with an odd leading dimension, for the forward sweeps (zeros right of the diagonal
-                    // inside the block; what lies above the block is never written and stays zero)
+                    // state block once more for the forward sweeps: as a packed lower triangle (tri), or with an odd leading
+                    // dimension (zeros right of the diagonal inside the block; what lies above the block is never written and
+                    // stays zero)
                     constexpr int nxk = n - nu, ldx = nxk | 1;
                     if (nxk > 0 && r >= nu)
                     {
 #pragma unroll
                         for (int q = 0; q < W; q++)
-                            if (j0 + q >= nu) Lxg[(r - nu) + ldx * (j0 + q - nu)] = xs[q];
+                        {
+                            if (PACK && j0 + q >= nu && rr >= q) Lxg[tri(nxk, r - nu, j0 + q - nu)] = xs[q];
+                            if (!PACK && j0 + q >= nu) Lxg[(r - nu) + ldx * (j0 + q - nu)] = xs[q];
+                        }
                     }
                 }
             }
@@ -1000,12 +1041,12 @@ struct Ker
             // (ML is zero above the diagonal for the whole sweep: fact_backward clears it, the panels write zeros there)
             {
                 double tt_[RPM > 0 ? RPM : 1];
-                cols_dot<nx1, nx1>(Lx, LDW, rb, tt_);
+                cols_dot<nx1, nx1>(Dense{Lx, LDW}, rb, tt_);
 #pragma unroll
                 for (int m = 0; m < CP; m++)
                     if (li + G * m < nx1) alb[li + G * m] = tt_[m];
                 fk_sync();
-                rows_dot<nx1, nx1>(Lx, LDW, alb, tt_);
+                rows_dot<nx1, nx1>(Dense{Lx, LDW}, alb, tt_);
                 double *Pb = v.w + sd.w_Pb;
 #pragma unroll
                 for (int m = 0; m < CP; m++)
@@ -1131,7 +1172,7 @@ struct Ker
                 for (int q = 0; q < 8; q++)
                 {
                     acc[m][q] = 0.0;
-                    h[m][q] = (q < w && r < n && r >= jt + q) ? fk_ldg(Hk + r + LDK * (jt + q)) : 0.0;
+                    h[m][q] = (q < w && r < n && r >= jt + q) ? fk_ldg(Hk + (PACK ? tri(n, r, jt + q) : r + LDK * (jt + q))) : 0.0;
                 }
             }
             if (MMA<nx1>::on)
@@ -1379,7 +1420,7 @@ struct Ker
         if (nx1 > 0)
         {
             double ap[RPM > 0 ? RPM : 1];
-            rows_dot<n, nx1>(MA, LDK, tmpx, ap);
+            rows_dot<n, nx1>(Dense{MA, LDK}, tmpx, ap);
 #pragma unroll
             for (int m = 0; m < RP; m++) x[m] += ap[m];
             fk_sync();
@@ -1487,7 +1528,7 @@ struct Ker
             bulk<0>(voff(MA), (size_t) A.kq[KIND] + (size_t) v.kk * A.kqs, evn(LDK * nx1));
         }
         if (nsolve > 0) bulk<2>(voff(LU), (size_t) v.kk * A.ws + sd.w_L, evn(n * nsolve));
-        if (nx1 > 0) bulk<2>(voff(ML), (size_t) v1.kk * A.ws + s1p->w_Lxx, evn((nx1 | 1) * nx1));
+        if (nx1 > 0) bulk<2>(voff(ML), (size_t) v1.kk * A.ws + s1p->w_Lxx, evn(PACK ? nx1 * (nx1 + 1) / 2 : (nx1 | 1) * nx1));
         stage_arm();
         wait_vec();
         const double *bs = RES, *rds = RES + (sd.res.d - sd.res.b), *rms = RES + (sd.res.m - sd.res.b);
@@ -1546,7 +1587,7 @@ struct Ker
         if (nx1 > 0)
         {
             double av[RPM > 0 ? RPM : 1];
-            cols_dot<n, nx1>(MA, LDK, vv, av);
+            cols_dot<n, nx1>(Dense{MA, LDK}, vv, av);
 #pragma unroll
             for (int m = 0; m < CP; m++)
             {
@@ -1649,10 +1690,9 @@ struct Ker
         if (nx1 > 0)
         {
             fk_sync();
-            const double *Lx = ML;                                          // Lxx of stage k+1, odd leading dimension, zero above the diagonal
-            constexpr int ldx = nx1 | 1;
+            const Lxx<nx1> Lx{ML};                                          // Lxx of stage k+1
             double tt_[RPM > 0 ? RPM : 1];
-            cols_dot<nx1, nx1>(Lx, ldx, x1, tt_);
+            cols_dot<nx1, nx1>(Lx, x1, tt_);
 #pragma unroll
             for (int m = 0; m < CP; m++)
             {
@@ -1661,7 +1701,7 @@ struct Ker
             }
             fk_sync();
             double *pi = v.w + sd.step.pi, *oa = v.w + sd.ires.b;
-            rows_dot<nx1, nx1>(Lx, ldx, tmp, tt_);
+            rows_dot<nx1, nx1>(Lx, tmp, tt_);
 #pragma unroll
             for (int m = 0; m < CP; m++)
             {

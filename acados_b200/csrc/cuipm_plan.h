@@ -154,16 +154,18 @@ inline bool fast_plan(const std::vector<StageDesc> &sd, const std::vector<int> &
     F.qp_stride = P.qp_stride; F.sol_stride = P.sol_stride; F.work_stride = P.work_stride; F.w_bkp = P.w_bkp;
     auto e = [](int n) { return (n + 1) & ~1; };
     F.nce = e(P.ncmax); F.nbe = e(P.nbgmax); F.ns2e = e(2 * P.nsmax); F.nve = e(P.nvsmax);
-    // kernel-side record: odd leading dimension >= nu+nx: row and column accesses in shared memory are both bank-conflict free
+    // kernel-side record: dynamics block with an odd leading dimension >= nu+nx (row and column accesses in shared memory are
+    // both bank-conflict free), Hessian as its packed lower triangle (n (n + 1) / 2 doubles) or with the same leading dimension
     const int NM = a.nx + a.nu;
     F.ld = NM | 1;
+    F.packed = fast_packed(a.nx, a.nu);
     unsigned o = 0;
     const StageDesc *three[3] = {&sd[0], &sd[1], &sd[N]};
     unsigned size[3];
     for (int t = 0; t < 3; t++)
     {
         const StageDesc &d = *three[t];
-        const unsigned szA = (unsigned) e(F.ld * d.nx1), szH = (unsigned) e(F.ld * d.n);
+        const unsigned szA = (unsigned) e(F.ld * d.nx1), szH = (unsigned) e(F.packed ? d.n * (d.n + 1) / 2 : F.ld * d.n);
         const unsigned szV = (d.q_stage + (unsigned) (d.q_stage_bytes / sizeof(double))) - d.q_b;
         F.kH[t] = szA; F.kV[t] = szA + szH;
         size[t] = szA + szH + (unsigned) e((int) szV);
@@ -175,8 +177,8 @@ inline bool fast_plan(const std::vector<StageDesc> &sd, const std::vector<int> &
 }
 
 // Caller's QP record -> kernel-side QP record of the throughput kernel (host version of the repack pass; the device version is
-// in cuipm_fast.cu): dynamics block with leading dimension F.ld, Hessian as a full symmetric matrix with leading dimension
-// F.ld, the vector part verbatim.
+// in cuipm_fast.cu): dynamics block with leading dimension F.ld, the lower triangle of the Hessian packed column by column
+// (fastk::tri) if F.packed, else the full symmetric matrix with leading dimension F.ld, the vector part verbatim.
 inline void repack_host(const FastArgs &F, const std::vector<StageDesc> &sd, const double *qp, double *qpk)
 {
     const int N = F.N, ld = F.ld;
@@ -188,8 +190,12 @@ inline void repack_host(const FastArgs &F, const std::vector<StageDesc> &sd, con
         for (int c = 0; c < d.nx1; c++)
             for (int r = 0; r < d.n; r++) o[r + ld * c] = qp[d.q_BAt + r + d.n * c];
         double *H = o + F.kH[kind];
-        for (int j = 0; j < d.n; j++)
-            for (int i = 0; i < d.n; i++) H[i + ld * j] = i >= j ? qp[d.q_RSQ + i + d.n * j] : qp[d.q_RSQ + j + d.n * i];
+        if (F.packed)
+            for (int j = 0, p = 0; j < d.n; j++)
+                for (int i = j; i < d.n; i++) H[p++] = qp[d.q_RSQ + i + d.n * j];
+        else
+            for (int j = 0; j < d.n; j++)
+                for (int i = 0; i < d.n; i++) H[i + ld * j] = i >= j ? qp[d.q_RSQ + i + d.n * j] : qp[d.q_RSQ + j + d.n * i];
         const unsigned nv = d.q_stage + (unsigned) (d.q_stage_bytes / sizeof(double)) - d.q_b;
         for (unsigned i = 0; i < nv; i++) o[F.kV[kind] + i] = qp[d.q_b + i];
     }
