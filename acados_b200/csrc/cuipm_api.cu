@@ -43,6 +43,9 @@ struct cuipm_solver
     float last_ms = 0.f;
     cuipm_opts last_opts{};
     FastPath fast;                           // throughput kernel (cuipm_fast.cu)
+    int spill = 0;                           // the generic kernel runs its global-scratch variant (P.spill, or tuning key "spill")
+    double *d_spill = nullptr;               // its scratch: spill_doubles(P) per QP, max_batch QPs (allocated at create if P.spill,
+                                             // else by the tuning key)
     cudaEvent_t evk0 = nullptr, evk1 = nullptr;   // around the throughput kernel of the last cuipm_solve_device call
     bool timed_fast = false;
 };
@@ -79,6 +82,7 @@ static int launch_batch(cuipm_solver *s, const LaunchArgs &a0, int slot, size_t 
     LaunchArgs a = a0;
     a.redo_list = nullptr;
     a.redo_count = nullptr;
+    a.spill = s->spill ? s->d_spill + spill_doubles(s->P) * lo : nullptr;
     const bool timed = slot == 0 && s->evk0;
     int rc = s->fast.enqueue(a, lo, slot, (void *) stream, launches, timed ? s->evk0 : nullptr, timed ? s->evk1 : nullptr);
     if (rc != CUIPM_OK) return rc;
@@ -115,6 +119,9 @@ extern "C" cuipm_solver *cuipm_create(const cuipm_shape *shape, int max_batch, i
     if (!alloc((void **) &s->d_sol, sizeof(double) * s->P.sol_stride * max_batch)) return fail();
     if (!alloc((void **) &s->d_work, sizeof(double) * s->P.work_stride * max_batch)) return fail();
     if (!alloc((void **) &s->d_info, sizeof(cuipm_info) * max_batch)) return fail();
+    // a separate buffer, not part of the work record: the getters, the sensitivities and the hand-back path read that layout
+    s->spill = s->P.spill;
+    if (s->spill && !alloc((void **) &s->d_spill, sizeof(double) * spill_doubles(s->P) * max_batch)) return fail();
     if (cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("cudaStreamCreate failed"); return fail(); }
     bool ok = cudaEventCreate(&s->ev0) == cudaSuccess && cudaEventCreate(&s->ev1) == cudaSuccess
               && cudaEventCreate(&s->evk0) == cudaSuccess && cudaEventCreate(&s->evk1) == cudaSuccess;
@@ -136,7 +143,7 @@ extern "C" void cuipm_destroy(cuipm_solver *s)
     cudaSetDevice(s->device);
     if (s->stream) cudaStreamSynchronize(s->stream);
     cudaFree(s->d_sd); cudaFree(s->d_ipool); cudaFree(s->d_qp); cudaFree(s->d_sol); cudaFree(s->d_work);
-    cudaFree(s->d_stat); cudaFree(s->d_info); cudaFree(s->d_seed); cudaFree(s->d_sens);
+    cudaFree(s->d_stat); cudaFree(s->d_info); cudaFree(s->d_seed); cudaFree(s->d_sens); cudaFree(s->d_spill);
     s->fast.destroy();
     if (s->ev0) cudaEventDestroy(s->ev0);
     if (s->ev1) cudaEventDestroy(s->ev1);
@@ -203,6 +210,17 @@ extern "C" int cuipm_set_tuning(cuipm_solver *s, const char *key, int value)
     if (!std::strcmp(key, "fast"))
     {
         s->fast.use = value != 0;
+        return CUIPM_OK;
+    }
+    if (!std::strcmp(key, "spill"))
+    {
+        // 1 runs the global-scratch variant on a shape that fits in shared memory too; 0 restores the plan's choice
+        if (value != 0 && !s->d_spill)
+        {
+            CK(cudaSetDevice(s->device));
+            CK(cudaMalloc(&s->d_spill, sizeof(double) * spill_doubles(s->P) * (size_t) s->max_batch));
+        }
+        s->spill = s->P.spill || value != 0;
         return CUIPM_OK;
     }
     set_error("unknown tuning key");
@@ -386,6 +404,7 @@ extern "C" int cuipm_sens_device(cuipm_solver *s, int nbatch, const double *d_qp
     a.P = s->P; a.sd = s->d_sd; a.ipool = s->d_ipool; a.qp = d_qp; a.sol = nullptr; a.work = s->d_work; a.info = nullptr;
     a.stat = nullptr; a.o = *opts; a.nbatch = nbatch; a.seed = d_seed; a.sens = d_sens; a.adjoint = adjoint != 0;
     a.redo_list = nullptr; a.redo_count = nullptr;
+    a.spill = s->spill ? s->d_spill : nullptr;
     CK(cudaEventRecord(s->ev0, s->stream));
     int e = launch_sens(a, s->warps, (void *) s->stream);
     if (e != 0) { set_error(std::string("kernel launch: ") + cudaGetErrorString((cudaError_t) e)); return CUIPM_ERR_CUDA; }

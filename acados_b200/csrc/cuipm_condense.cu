@@ -26,13 +26,15 @@ struct CtaExec
     }
 };
 
-template <int MODE>
-__global__ void condense_kernel(Plan P, const double *qp, double *qp2, double *tbuf, int nbatch)
+// GSCR: the scratch of a block that needs more than 227 KB is QP q's slice of a device buffer (gscr, scr_stride doubles per QP)
+template <int MODE, bool GSCR>
+__global__ void condense_kernel(Plan P, const double *qp, double *qp2, double *tbuf, double *gscr, size_t scr_stride, int nbatch)
 {
-    extern __shared__ double scr[];
+    extern __shared__ double sscr[];
     const int q = blockIdx.x;
     if (q >= nbatch) return;
     CtaExec ex;
+    double *scr = GSCR ? gscr + (size_t) q * scr_stride : sscr;
     condense_one<MODE>(ex, P, qp + (size_t) q * P.o.qp_stride, qp2 + (size_t) q * P.c.qp_stride, scr,
                        MODE == COND_ALL ? nullptr : tbuf + (size_t) q * P.t_stride);
 }
@@ -55,9 +57,16 @@ struct cuipm_condenser
     Plan P{};
     int *d_i = nullptr;
     unsigned *d_u = nullptr;
-    size_t smem = 0;
+    size_t smem = 0;              // dynamic shared memory of the condensing kernels (0 with the scratch in global memory)
+    size_t smem_exp = 0;          // ... and of the expansion kernel
     double *d_t = nullptr;        // T_j of the QPs of the last lhs pass (t_stride doubles per QP)
     int t_cap = 0, t_valid = 0;   // QPs the buffer holds / QPs the last lhs pass filled
+    // condensed blocks whose scratch exceeds 227 KB: the scratch of QP q is d_scr + q * scr_stride (grown on demand, like d_t;
+    // calls of one condenser therefore go on one stream, or do not overlap)
+    bool gscr = false;
+    size_t scr_stride = 0;
+    double *d_scr = nullptr;
+    int scr_cap = 0;
 };
 
 #define CKC(call)                                                                                       \
@@ -70,6 +79,29 @@ struct cuipm_condenser
         }                                                                                               \
     } while (0)
 
+// launches condense_kernel<MODE> with the scratch where the plan needs it
+template <int MODE>
+static int launch_condense(cuipm_condenser *c, int nbatch, const double *d_qp, double *d_qp_cond, double *tbuf, cudaStream_t stream)
+{
+    if (!c->gscr)
+    {
+        condense_kernel<MODE, false><<<nbatch, 128, c->smem, stream>>>(c->P, d_qp, d_qp_cond, tbuf, nullptr, 0, nbatch);
+        CKC(cudaGetLastError());
+        return CUIPM_OK;
+    }
+    if (c->scr_cap < nbatch)
+    {
+        CKC(cudaStreamSynchronize(stream));
+        cudaFree(c->d_scr);
+        c->d_scr = nullptr; c->scr_cap = 0;
+        CKC(cudaMalloc(&c->d_scr, sizeof(double) * c->scr_stride * (size_t) nbatch));
+        c->scr_cap = nbatch;
+    }
+    condense_kernel<MODE, true><<<nbatch, 128, 0, stream>>>(c->P, d_qp, d_qp_cond, tbuf, c->d_scr, c->scr_stride, nbatch);
+    CKC(cudaGetLastError());
+    return CUIPM_OK;
+}
+
 extern "C" void cuipm_condenser_destroy(cuipm_condenser *c)
 {
     if (!c) return;
@@ -77,6 +109,7 @@ extern "C" void cuipm_condenser_destroy(cuipm_condenser *c)
     cudaFree(c->d_i);
     cudaFree(c->d_u);
     cudaFree(c->d_t);
+    cudaFree(c->d_scr);
     delete c;
 }
 
@@ -102,11 +135,19 @@ extern "C" cuipm_condenser *cuipm_condenser_create(const cuipm_shape *shape, int
     }
     c->P = c->hp.plan(c->d_i, c->d_u);
     c->smem = sizeof(double) * (size_t) scratch_doubles(c->P);
-    if (c->smem > 227 * 1024) { set_error("condensed stage too large for the shared-memory scratch"); cuipm_condenser_destroy(c); return nullptr; }
-    cudaFuncSetAttribute(condense_kernel<COND_ALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem);
-    cudaFuncSetAttribute(condense_kernel<COND_LHS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem);
-    cudaFuncSetAttribute(condense_kernel<COND_RHS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem);
-    cudaFuncSetAttribute(expand_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem);
+    c->smem_exp = c->smem;
+    if (c->smem > 227 * 1024)
+    {
+        // the scratch goes to a device buffer, one slice per QP; the expansion needs only its first 4 nxmax doubles
+        c->gscr = true;
+        c->scr_stride = (size_t) ((scratch_doubles(c->P) + 1) & ~1);
+        c->smem = 0;
+        c->smem_exp = sizeof(double) * (size_t) expand_scratch_doubles(c->P);
+    }
+    cudaFuncSetAttribute(condense_kernel<COND_ALL, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem);
+    cudaFuncSetAttribute(condense_kernel<COND_LHS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem);
+    cudaFuncSetAttribute(condense_kernel<COND_RHS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem);
+    cudaFuncSetAttribute(expand_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem_exp);
     return c;
 }
 
@@ -119,9 +160,7 @@ extern "C" int cuipm_condense_device(cuipm_condenser *c, int nbatch, const doubl
     CKC(cudaSetDevice(c->device));
     // the masks of a fresh record are 1 and untouched entries of d / Z / z are 0 in the reference's layout: clear, then fill
     CKC(cudaMemsetAsync(d_qp_cond, 0, sizeof(double) * c->hp.lc->qp_stride * (size_t) nbatch, (cudaStream_t) stream));
-    condense_kernel<COND_ALL><<<nbatch, 128, c->smem, (cudaStream_t) stream>>>(c->P, d_qp, d_qp_cond, nullptr, nbatch);
-    CKC(cudaGetLastError());
-    return CUIPM_OK;
+    return launch_condense<COND_ALL>(c, nbatch, d_qp, d_qp_cond, nullptr, (cudaStream_t) stream);
 }
 
 // The split of acados' xcond solver (ocp_qp_xcond_solver.c:591-669: condense_lhs in the preparation phase of an SQP-RTI step,
@@ -142,8 +181,8 @@ extern "C" int cuipm_condense_lhs_device(cuipm_condenser *c, int nbatch, const d
         c->t_cap = nbatch;
     }
     CKC(cudaMemsetAsync(d_qp_cond, 0, sizeof(double) * c->hp.lc->qp_stride * (size_t) nbatch, (cudaStream_t) stream));
-    condense_kernel<COND_LHS><<<nbatch, 128, c->smem, (cudaStream_t) stream>>>(c->P, d_qp, d_qp_cond, c->d_t, nbatch);
-    CKC(cudaGetLastError());
+    const int rc = launch_condense<COND_LHS>(c, nbatch, d_qp, d_qp_cond, c->d_t, (cudaStream_t) stream);
+    if (rc != CUIPM_OK) return rc;
     c->t_valid = nbatch;
     return CUIPM_OK;
 }
@@ -154,9 +193,7 @@ extern "C" int cuipm_condense_rhs_device(cuipm_condenser *c, int nbatch, const d
     if (nbatch > c->t_valid) { set_error("cuipm_condense_rhs_device: no lhs pass for this many QPs (call cuipm_condense_lhs_device first)"); return CUIPM_ERR_INVALID; }
     if (nbatch == 0) return CUIPM_OK;
     CKC(cudaSetDevice(c->device));
-    condense_kernel<COND_RHS><<<nbatch, 128, c->smem, (cudaStream_t) stream>>>(c->P, d_qp, d_qp_cond, c->d_t, nbatch);
-    CKC(cudaGetLastError());
-    return CUIPM_OK;
+    return launch_condense<COND_RHS>(c, nbatch, d_qp, d_qp_cond, c->d_t, (cudaStream_t) stream);
 }
 
 extern "C" int cuipm_expand_device(cuipm_condenser *c, int nbatch, const double *d_qp, const double *d_sol_cond, double *d_sol, void *stream)
@@ -165,7 +202,7 @@ extern "C" int cuipm_expand_device(cuipm_condenser *c, int nbatch, const double 
     if (nbatch == 0) return CUIPM_OK;
     CKC(cudaSetDevice(c->device));
     CKC(cudaMemsetAsync(d_sol, 0, sizeof(double) * c->hp.lo->sol_stride * (size_t) nbatch, (cudaStream_t) stream));
-    expand_kernel<<<nbatch, 128, c->smem, (cudaStream_t) stream>>>(c->P, d_qp, d_sol_cond, d_sol, nbatch);
+    expand_kernel<<<nbatch, 128, c->smem_exp, (cudaStream_t) stream>>>(c->P, d_qp, d_sol_cond, d_sol, nbatch);
     CKC(cudaGetLastError());
     return CUIPM_OK;
 }

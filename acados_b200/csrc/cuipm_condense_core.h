@@ -9,7 +9,8 @@
 // first stage's state bounds stay boxes, inner state bounds / general constraints become general constraints with shifted bounds.
 //
 // Data parallelism inside a QP: every phase is "thread t handles elements t, t+NT, ... of an output array" (column-major, so
-// consecutive threads touch consecutive addresses of the records); the small operands T, c, Q T live in the CTA's scratch.
+// consecutive threads touch consecutive addresses of the records); the small operands T, c, Q T live in the CTA's scratch
+// (shared memory, or the QP's slice of a device buffer where the blocks need more than 227 KB: cuipm_condense.cu).
 #ifndef CUIPM_CONDENSE_CORE_H_
 #define CUIPM_CONDENSE_CORE_H_
 
@@ -50,6 +51,8 @@ struct Plan
 enum { COND_ALL = 0, COND_LHS = 1, COND_RHS = 2 };
 
 CC_HD inline int scratch_doubles(const Plan &P) { return 2 * P.nxmax * P.n2max + 4 * P.nxmax + 2 * P.n2max + 16; }
+// the part of it expand_one uses (xv, xn, pv, pn)
+CC_HD inline int expand_scratch_doubles(const Plan &P) { return 4 * P.nxmax; }
 
 // symmetric access to the lower-stored Hessian block of the ORIGINAL record (column-major, ld n)
 CC_HD inline double hsym(const double *H, int n, int i, int j) { return i >= j ? H[i + n * j] : H[j + n * i]; }

@@ -43,12 +43,22 @@ struct ProbDesc
     int mid_nx, mid_nu;                                    // (nx, nu) shared by stages 1..N-1 and nx of stage N, or 0,0 if not uniform
     unsigned w_lq;                                         // work record: nmax x (nbgmax + nxmax) scratch of the LQ refactorisation
     unsigned w_bkp;                                        // work record: lam, t of the iterate of the last factorisation, in a record of the solution layout
-    int pad_;
+    int spill;                                             // 1: the stage-block buffers (sm_M, sm_A, sm_AL, sm_C) do not fit in shared memory
+                                                           //    next to sm_V; the generic kernel keeps them in a per-QP slice of a device
+                                                           //    scratch buffer (spill_doubles(P) doubles per QP) instead
     size_t qp_stride, sol_stride, work_stride;
     // shared-memory carve (doubles)
     int sm_M, sm_A, sm_AL, sm_C, sm_V;
     int sm_total;
 };
+
+#ifdef __CUDACC__
+#define CUIPM_HD __host__ __device__
+#else
+#define CUIPM_HD
+#endif
+// doubles of the stage-block buffers of one QP, in the order sm_M, sm_A, sm_AL, sm_C (even: 16-byte aligned slices)
+CUIPM_HD inline size_t spill_doubles(const ProbDesc &P) { return (size_t) P.sm_M + P.sm_A + P.sm_AL + P.sm_C; }
 
 struct LaunchArgs
 {
@@ -70,6 +80,9 @@ struct LaunchArgs
     // both null for a plain launch over the whole batch
     const int *redo_list;
     const int *redo_count;
+    // global-scratch variant of the generic kernel: stage-block buffers of QP q at spill + q * spill_doubles(P) (same QP index
+    // as qp / sol / work); null: the buffers are in shared memory
+    double *spill;
 };
 
 // Arguments of the throughput kernel (cuipm_fast.cu): shapes whose interior stages are uniform need three stage

@@ -26,6 +26,12 @@ __device__ __forceinline__ int ev(int n) { return (n + 1) & ~1; }
 // Per-CTA solver context.  It lives in static shared memory and is reached by name (never through a pointer), and the
 // dynamic shared memory is reached through the extern array below, so that every on-chip access compiles to LDS/STS
 // with 32-bit addressing instead of generic loads.
+//
+// Global-scratch variant (Ker<..., SPILL = true>, for shapes whose buffers exceed 227 KB of shared memory): the stage-block
+// buffers SM_, SA_, SAL_, SC_ are this QP's slice of a device scratch buffer (Ctx::spx), the vector area SV_ and the context
+// stay on chip.  The sweeps perform the same arithmetic in the same order on the same operands; only the copies into those
+// buffers change, from LDGSTS (cp.async needs a shared destination) to plain loads and stores (cpb8 / cpvb).  __syncthreads /
+// __syncwarp order global memory among the CTA's threads as they order shared memory.
 struct Ctx
 {
     ProbDesc P;
@@ -43,16 +49,19 @@ struct Ctx
 #ifdef CUIPM_PROFILE
     long long prof[16];   // cycles per pass kind (thread 0): 0 res, 1 res_lin, 2 fact_backward, 3 forward, 4 solve_backward, 5 vector passes
 #endif
+    double *spx;          // global-scratch variant: this QP's slice of the scratch buffer (spill_doubles(P) doubles)
 };
 __shared__ Ctx g_cx;
 __shared__ double g_red[8];
 extern __shared__ __align__(16) double g_smem[];
 #define CX g_cx
-#define SM_ (g_smem)
-#define SA_ (g_smem + CX.P.sm_M)
-#define SAL_ (g_smem + CX.P.sm_M + CX.P.sm_A)
-#define SC_ (g_smem + CX.P.sm_M + CX.P.sm_A + CX.P.sm_AL)
-#define SV_ (g_smem + CX.P.sm_M + CX.P.sm_A + CX.P.sm_AL + CX.P.sm_C)
+// SPILL is the template parameter of Ker (and of the kernels): a compile-time constant, so the on-chip variant's addresses
+// are those of the plain extern array
+#define SM_ (SPILL ? CX.spx : g_smem)
+#define SA_ (SM_ + CX.P.sm_M)
+#define SAL_ (SM_ + CX.P.sm_M + CX.P.sm_A)
+#define SC_ (SM_ + CX.P.sm_M + CX.P.sm_A + CX.P.sm_AL)
+#define SV_ (SPILL ? g_smem : g_smem + CX.P.sm_M + CX.P.sm_A + CX.P.sm_AL + CX.P.sm_C)
 #ifdef CUIPM_PROFILE
 #define PROF_T0() long long t0_ = clock64()
 #define PROF_ADD(slot) do { if (tid == 0) CX.prof[slot] += clock64() - t0_; t0_ = clock64(); } while (0)
@@ -83,7 +92,7 @@ struct SDims   // interior stage k (1 <= k <= N-2) of a horizon with uniform (nx
     __device__ __forceinline__ constexpr int n1(const StageDesc &) const { return NX_ + NU_; }
 };
 
-template <int W, int SNX, int SNU>
+template <int W, int SNX, int SNU, bool SPILL>
 struct Ker
 {
     static constexpr int NT = 32 * W;
@@ -239,6 +248,20 @@ struct Ker
     __device__ __forceinline__ void cpv(double *sdst, const double *gsrc, int n) const
     {
         for (int i = tid; i < n; i += NT) cpa8(sdst + i, gsrc + i);
+    }
+    // the same two copies into the stage-block buffers (SM_, SAL_, SC_): asynchronous into shared memory, plain load and store
+    // into the global scratch of the SPILL variant (RO: the source is a QP record, read-only for the whole launch)
+    template <bool RO>
+    __device__ __forceinline__ void cpb8(double *dst, const double *gsrc) const
+    {
+        if (SPILL) *dst = ldv<RO>(gsrc);
+        else cpa8(dst, gsrc);
+    }
+    __device__ __forceinline__ void cpvb(double *dst, const double *gsrc, int n) const
+    {
+        if (SPILL)
+            for (int i = tid; i < n; i += NT) dst[i] = ldv<false>(gsrc + i);
+        else cpv(dst, gsrc, n);
     }
     // stage descriptor k -> ring slot k & 3, asynchronously (LDGSTS); desc_wait() + a barrier make it visible
     __device__ __forceinline__ void desc_fetch(int k)
@@ -630,9 +653,9 @@ struct Ker
                 for (int r = tid; r <= n; r += NT)
                 {
                     if (r < n)
-                        for (int c = 0; c < nx1; c++) cpa8(SAL_ + r + ldal * c, Ag + r + n * c);
+                        for (int c = 0; c < nx1; c++) cpb8<true>(SAL_ + r + ldal * c, Ag + r + n * c);
                     else
-                        for (int c = 0; c < nx1; c++) cpa8(SAL_ + n + ldal * c, b_ + c);
+                        for (int c = 0; c < nx1; c++) cpb8<false>(SAL_ + n + ldal * c, b_ + c);
                 }
             }
             if (k > 0)
@@ -1158,9 +1181,9 @@ struct Ker
                 // pure copies first, as asynchronous global -> shared copies (all in flight at once) ...
                 cpv(v, rg(rhs, s), n);
                 if (ns > 0) cpv(Zi, CX.wk + s.w_Zsi, 2 * ns);
-                cpv(Ls, Lg, n * nsolve);
-                cpv(Lis, Li, nsolve);
-                if (k < N && use_Pb) cpv(pbs, CX.wk + s.w_Pb, nx1);
+                cpvb(Ls, Lg, n * nsolve);
+                cpvb(Lis, Li, nsolve);
+                if (k < N && use_Pb) cpvb(pbs, CX.wk + s.w_Pb, nx1);
                 // ... then the constraint quantities through registers while those are in flight
                 const double *gl = CX.sol + s.sol.lam, *gt = CX.sol + s.sol.t, *grd = rd(rhs, s), *gm = CX.qp + s.q_dmask;
                 double *grm = rm(rhs, s);
@@ -1987,8 +2010,12 @@ struct Ker
 #ifndef CUIPM_MINB
 #define CUIPM_MINB 16
 #endif
-template <int W, int SNX, int SNU>
-__global__ void __launch_bounds__(32 * W, (W == 1 ? CUIPM_MINB : (W == 2 ? 8 : 4))) cuipm_solve_kernel(const LaunchArgs a)
+// resident CTAs per SM the register allocation is bounded for: the on-chip variant 16 / 8 / 4 (W = 1 / 2 / 4); the global-scratch
+// variant 1, so that its register allocation is unconstrained (no local-memory spills): its shapes are too large for more
+// than a few CTAs per SM to help, and they run from L2 anyway
+#define CUIPM_MIN_CTAS(W, SPILL) ((SPILL) ? 1 : ((W) == 1 ? CUIPM_MINB : ((W) == 2 ? 8 : 4)))
+template <int W, int SNX, int SNU, bool SPILL>
+__global__ void __launch_bounds__(32 * W, CUIPM_MIN_CTAS(W, SPILL)) cuipm_solve_kernel(const LaunchArgs a)
 {
     if (threadIdx.x == 0)
     {
@@ -1997,7 +2024,7 @@ __global__ void __launch_bounds__(32 * W, (W == 1 ? CUIPM_MINB : (W == 2 ? 8 : 4
         CX.ipool = a.ipool;
         CX.o = a.o;
     }
-    Ker<W, SNX, SNU> K;
+    Ker<W, SNX, SNU, SPILL> K;
     // second pass behind the throughput kernel: only the QPs it handed back
     const int nq = a.redo_count ? *a.redo_count : a.nbatch;
     for (int i = blockIdx.x; i < nq; i += gridDim.x)
@@ -2008,6 +2035,8 @@ __global__ void __launch_bounds__(32 * W, (W == 1 ? CUIPM_MINB : (W == 2 ? 8 : 4
             CX.qp = a.qp + (size_t) q * a.P.qp_stride;
             CX.sol = a.sol + (size_t) q * a.P.sol_stride;
             CX.wk = a.work + (size_t) q * a.P.work_stride;
+            // by QP, not by CTA: the chunks of a host solve run concurrently, each with its own part of the scratch
+            if (SPILL) CX.spx = a.spill + (size_t) q * spill_doubles(a.P);
         }
         K.sync();
         if (a.redo_list && a.o.warm_start >= 2) K.restore_warm_start();
@@ -2016,8 +2045,8 @@ __global__ void __launch_bounds__(32 * W, (W == 1 ? CUIPM_MINB : (W == 2 ? 8 : 4
     }
 }
 
-template <int W>
-__global__ void __launch_bounds__(32 * W, (W == 1 ? CUIPM_MINB : (W == 2 ? 8 : 4))) cuipm_sens_kernel(const LaunchArgs a)
+template <int W, bool SPILL>
+__global__ void __launch_bounds__(32 * W, CUIPM_MIN_CTAS(W, SPILL)) cuipm_sens_kernel(const LaunchArgs a)
 {
     if (threadIdx.x == 0)
     {
@@ -2028,7 +2057,7 @@ __global__ void __launch_bounds__(32 * W, (W == 1 ? CUIPM_MINB : (W == 2 ? 8 : 4
         CX.mask_constr = 0;      // the reference's sensitivity substitution does not mask
         CX.nc_mask_inv = 0.0;
     }
-    Ker<W, 0, 0> K;
+    Ker<W, 0, 0, SPILL> K;
     for (int q = blockIdx.x; q < a.nbatch; q += gridDim.x)
     {
         if (threadIdx.x == 0)
@@ -2036,6 +2065,7 @@ __global__ void __launch_bounds__(32 * W, (W == 1 ? CUIPM_MINB : (W == 2 ? 8 : 4
             CX.qp = a.qp + (size_t) q * a.P.qp_stride;
             CX.wk = a.work + (size_t) q * a.P.work_stride;
             CX.sol = CX.wk + a.P.w_bkp;      // lam, t of the iterate the factorisation belongs to
+            if (SPILL) CX.spx = a.spill + (size_t) q * spill_doubles(a.P);
         }
         K.sync();
         K.sens(a.seed + (size_t) q * a.P.sol_stride, a.sens + (size_t) q * a.P.sol_stride, a.adjoint);
@@ -2045,26 +2075,32 @@ __global__ void __launch_bounds__(32 * W, (W == 1 ? CUIPM_MINB : (W == 2 ? 8 : 4
 
 }  // namespace
 
-// dynamic shared memory (bytes) the kernel needs for P
-static size_t smem_bytes(const ProbDesc &P) { return sizeof(double) * (size_t) P.sm_total; }
+// dynamic shared memory (bytes) the kernel needs for P: every buffer, or the vector area alone in the global-scratch variant
+static size_t smem_bytes(const LaunchArgs &a) { return sizeof(double) * (size_t) (a.spill ? a.P.sm_V : a.P.sm_total); }
 
-template <int W, int SNX, int SNU>
+template <int W, int SNX, int SNU, bool SPILL = false>
 static cudaError_t launch_one(const LaunchArgs &a, size_t smem, cudaStream_t stream)
 {
-    cudaError_t err = cudaFuncSetAttribute(cuipm_solve_kernel<W, SNX, SNU>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+    cudaError_t err = cudaFuncSetAttribute(cuipm_solve_kernel<W, SNX, SNU, SPILL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
     if (err != cudaSuccess) return err;
     // behind the throughput kernel only a few QPs are left: a small grid whose blocks walk the hand-back list
     const int grid = a.redo_list ? (a.nbatch < 1184 ? a.nbatch : 1184) : a.nbatch;
-    cuipm_solve_kernel<W, SNX, SNU><<<grid, 32 * W, smem, stream>>>(a);
+    cuipm_solve_kernel<W, SNX, SNU, SPILL><<<grid, 32 * W, smem, stream>>>(a);
     return cudaGetLastError();
 }
 
 // (nx, nu) pairs with a compile-time specialisation of the interior stages (BASELINE.json configs 1-4); any other
-// shape runs the generic path
+// shape runs the generic path.  With a scratch buffer (a.spill): the global-scratch variant, generic dimensions only.
 int launch_solve(const LaunchArgs &a, int warps, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t) stream_;
-    const size_t smem = smem_bytes(a.P);
+    const size_t smem = smem_bytes(a);
+    if (a.spill)
+    {
+        if (warps <= 1) return (int) launch_one<1, 0, 0, true>(a, smem, stream);
+        if (warps == 2) return (int) launch_one<2, 0, 0, true>(a, smem, stream);
+        return (int) launch_one<4, 0, 0, true>(a, smem, stream);
+    }
     if (warps <= 1)
     {
         const int nx = a.P.mid_nx, nu = a.P.mid_nu;
@@ -2078,22 +2114,28 @@ int launch_solve(const LaunchArgs &a, int warps, void *stream_)
     return (int) launch_one<4, 0, 0>(a, smem, stream);
 }
 
-template <int W>
+template <int W, bool SPILL>
 static cudaError_t launch_sens_one(const LaunchArgs &a, size_t smem, cudaStream_t stream)
 {
-    cudaError_t err = cudaFuncSetAttribute(cuipm_sens_kernel<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+    cudaError_t err = cudaFuncSetAttribute(cuipm_sens_kernel<W, SPILL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
     if (err != cudaSuccess) return err;
-    cuipm_sens_kernel<W><<<a.nbatch, 32 * W, smem, stream>>>(a);
+    cuipm_sens_kernel<W, SPILL><<<a.nbatch, 32 * W, smem, stream>>>(a);
     return cudaGetLastError();
+}
+
+template <bool SPILL>
+static cudaError_t launch_sens_w(const LaunchArgs &a, int warps, size_t smem, cudaStream_t stream)
+{
+    if (warps <= 1) return launch_sens_one<1, SPILL>(a, smem, stream);
+    if (warps == 2) return launch_sens_one<2, SPILL>(a, smem, stream);
+    return launch_sens_one<4, SPILL>(a, smem, stream);
 }
 
 int launch_sens(const LaunchArgs &a, int warps, void *stream_)
 {
     cudaStream_t stream = (cudaStream_t) stream_;
-    const size_t smem = smem_bytes(a.P);
-    if (warps <= 1) return (int) launch_sens_one<1>(a, smem, stream);
-    if (warps == 2) return (int) launch_sens_one<2>(a, smem, stream);
-    return (int) launch_sens_one<4>(a, smem, stream);
+    const size_t smem = smem_bytes(a);
+    return (int) (a.spill ? launch_sens_w<true>(a, warps, smem, stream) : launch_sens_w<false>(a, warps, smem, stream));
 }
 
 }  // namespace cuipm

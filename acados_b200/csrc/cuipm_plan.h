@@ -88,6 +88,12 @@ inline int build_plan(const cuipm_shape *sh, const cuipm_layout *l, std::vector<
     P.w_bkp = (unsigned) w;
     w += plan_ev2u(l->sol_stride);
     if (w >= (size_t) 1 << 32 || l->qp_stride >= (size_t) 1 << 32) { err = "QP record too large for 32-bit offsets"; return CUIPM_ERR_TOO_LARGE; }
+    // the stage-block buffers below are indexed with int offsets (on chip or in the scratch slice of one QP)
+    if ((size_t) (P.nmax + 2) * ((size_t) P.nmax + P.nxmax + 3 * (size_t) P.ngmax) + 4 * (size_t) P.ncmax + 64 >= (size_t) 1 << 31)
+    {
+        err = "stage blocks too large for 32-bit offsets";
+        return CUIPM_ERR_TOO_LARGE;
+    }
     P.qp_stride = l->qp_stride; P.sol_stride = l->sol_stride; P.work_stride = w;
     auto e = [](int n) { return (n + 1) & ~1; };
     // leading dimensions used on chip: nmax|1 (odd, conflict-free row/column access) or even(nmax+1) (factorisation:
@@ -106,7 +112,14 @@ inline int build_plan(const cuipm_shape *sh, const cuipm_layout *l, std::vector<
         P.sm_V = std::max(std::max(std::max(v_res, v_fwd), std::max(v_fact, v_slv)), v_init) + 8;
     }
     P.sm_total = P.sm_M + P.sm_A + P.sm_AL + P.sm_C + P.sm_V;
-    if (sizeof(double) * (size_t) P.sm_total > 227 * 1024) { err = "stage dimensions need more than 227 KB of shared memory"; return CUIPM_ERR_TOO_LARGE; }
+    // Shapes whose buffers exceed the 227 KB of shared memory a block may have run the generic kernel's global-scratch
+    // variant: the stage-block buffers move to a device scratch buffer, the vector area stays on chip.
+    P.spill = sizeof(double) * (size_t) P.sm_total > 227 * 1024;
+    if (P.spill && sizeof(double) * (size_t) P.sm_V > 227 * 1024)
+    {
+        err = "stage dimensions need more than 227 KB of shared memory for the solver's vectors alone";
+        return CUIPM_ERR_TOO_LARGE;
+    }
     return CUIPM_OK;
 }
 

@@ -46,7 +46,9 @@ enum cuipm_error {
     CUIPM_ERR_INVALID = -1,     /* bad argument / unsupported option value */
     CUIPM_ERR_CUDA = -2,        /* CUDA runtime error (message via cuipm_last_error) */
     CUIPM_ERR_NO_DEVICE = -3,   /* no CUDA device: there is NO CPU fallback */
-    CUIPM_ERR_TOO_LARGE = -4    /* stage dimensions exceed what the kernel supports */
+    CUIPM_ERR_TOO_LARGE = -4    /* stage dimensions exceed what the kernel supports: the solver's vectors alone need more than
+                                 * 227 KB of shared memory, or a record needs offsets beyond 32 bits.  (Stage blocks that do not
+                                 * fit in shared memory are not refused: they go to a per-QP device scratch buffer.) */
 };
 
 /* modes: external/hpipm/include/hpipm_common.h (enum hpipm_mode) */
@@ -296,8 +298,11 @@ int cuipm_last_handed_back(cuipm_solver *s);
 /* launch tuning without a reference counterpart: key "warps" = warps cooperating on one QP in the generic kernel (1, 2 or 4;
  * the default is chosen from the stage dimensions); key "pipe" = chunks (1..8, default 8) the host entry splits a batch into
  * so that the copies of one chunk overlap the solve of the others; key "fast" = 0 keeps eligible shapes off the throughput
- * kernel (several QPs per warp, acados_b200/csrc/cuipm_fast.cu).  Results do not depend on any of them beyond
- * floating-point summation order. */
+ * kernel (several QPs per warp, acados_b200/csrc/cuipm_fast.cu); key "spill" = 1 runs the generic kernel's global-scratch
+ * variant (stage-block buffers in a per-QP device scratch buffer, allocated on first use) on a shape that fits in shared
+ * memory, 0 restores the default -- a test hook like "fast": the variant is chosen by itself exactly for the shapes that do
+ * not fit, and gives the same results bit for bit.  Results do not depend on any of them beyond floating-point summation
+ * order. */
 int cuipm_set_tuning(cuipm_solver *s, const char *key, int value);
 
 #ifdef __cplusplus
