@@ -23,7 +23,6 @@ struct cuipm_solver
 {
     int device = 0;
     int max_batch = 0;
-    int warps = 1;
     cuipm_layout *layout = nullptr;
     ProbDesc P{};
     std::vector<StageDesc> sd_host;
@@ -42,23 +41,38 @@ struct cuipm_solver
     int pending = 0;                         // an asynchronous host solve has been enqueued and not waited for
     float last_ms = 0.f;
     cuipm_opts last_opts{};
+    GenericPath generic;                     // generic kernel (cuipm_kernel.cu)
     FastPath fast;                           // throughput kernel (cuipm_fast.cu)
-    int spill = 0;                           // the generic kernel runs its global-scratch variant (P.spill, or tuning key "spill")
-    double *d_spill = nullptr;               // its scratch: spill_doubles(P) per QP, max_batch QPs (allocated at create if P.spill,
-                                             // else by the tuning key)
     cudaEvent_t evk0 = nullptr, evk1 = nullptr;   // around the throughput kernel of the last cuipm_solve_device call
     bool timed_fast = false;
 };
 
-#define CK(call)                                                                                        \
-    do {                                                                                                \
-        cudaError_t e_ = (call);                                                                        \
-        if (e_ != cudaSuccess)                                                                          \
-        {                                                                                               \
-            set_error(std::string(#call) + ": " + cudaGetErrorString(e_));                              \
-            return CUIPM_ERR_CUDA;                                                                      \
-        }                                                                                               \
-    } while (0)
+namespace cuipm {
+
+int smem_limit(const void *kernel, size_t *bytes)
+{
+    int device = 0, optin = 0;
+    cudaFuncAttributes fa{};
+    CK(cudaGetDevice(&device));
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+    CK(cudaFuncGetAttributes(&fa, kernel));
+    *bytes = (size_t) optin - fa.sharedSizeBytes;
+    return CUIPM_OK;
+}
+
+int set_dynamic_smem(const void *kernel, size_t bytes)
+{
+    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) bytes));
+    return CUIPM_OK;
+}
+
+int cuda_error(const std::string &what, int err)
+{
+    set_error(what + ": " + cudaGetErrorString((cudaError_t) err));
+    return CUIPM_ERR_CUDA;
+}
+
+}  // namespace cuipm
 
 static int build_desc(cuipm_solver *s, const cuipm_shape *sh)
 {
@@ -66,6 +80,8 @@ static int build_desc(cuipm_solver *s, const cuipm_shape *sh)
     std::string err;
     int rc = build_plan(sh, s->layout, s->sd_host, ipool, s->P, err);
     if (rc != CUIPM_OK) { set_error(err); return rc; }
+    rc = s->generic.create(s->P, s->max_batch, s->device);
+    if (rc != CUIPM_OK) return rc;
     const int N = sh->N;
     CK(cudaMalloc(&s->d_sd, sizeof(StageDesc) * (N + 1)));
     CK(cudaMemcpy(s->d_sd, s->sd_host.data(), sizeof(StageDesc) * (N + 1), cudaMemcpyHostToDevice));
@@ -82,13 +98,12 @@ static int launch_batch(cuipm_solver *s, const LaunchArgs &a0, int slot, size_t 
     LaunchArgs a = a0;
     a.redo_list = nullptr;
     a.redo_count = nullptr;
-    a.spill = s->spill ? s->d_spill + spill_doubles(s->P) * lo : nullptr;
     const bool timed = slot == 0 && s->evk0;
     int rc = s->fast.enqueue(a, lo, slot, (void *) stream, launches, timed ? s->evk0 : nullptr, timed ? s->evk1 : nullptr);
     if (rc != CUIPM_OK) return rc;
     if (timed && a.redo_count) s->timed_fast = true;
-    rc = launch_solve(a, s->warps, (void *) stream);
-    if (rc != 0) { set_error(std::string("kernel launch: ") + cudaGetErrorString((cudaError_t) rc)); return CUIPM_ERR_CUDA; }
+    rc = s->generic.solve(a, lo, (void *) stream);
+    if (rc != CUIPM_OK) return rc;
     (*launches)++;
     return CUIPM_OK;
 }
@@ -119,9 +134,6 @@ extern "C" cuipm_solver *cuipm_create(const cuipm_shape *shape, int max_batch, i
     if (!alloc((void **) &s->d_sol, sizeof(double) * s->P.sol_stride * max_batch)) return fail();
     if (!alloc((void **) &s->d_work, sizeof(double) * s->P.work_stride * max_batch)) return fail();
     if (!alloc((void **) &s->d_info, sizeof(cuipm_info) * max_batch)) return fail();
-    // a separate buffer, not part of the work record: the getters, the sensitivities and the hand-back path read that layout
-    s->spill = s->P.spill;
-    if (s->spill && !alloc((void **) &s->d_spill, sizeof(double) * spill_doubles(s->P) * max_batch)) return fail();
     if (cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking) != cudaSuccess) { set_error("cudaStreamCreate failed"); return fail(); }
     bool ok = cudaEventCreate(&s->ev0) == cudaSuccess && cudaEventCreate(&s->ev1) == cudaSuccess
               && cudaEventCreate(&s->evk0) == cudaSuccess && cudaEventCreate(&s->evk1) == cudaSuccess;
@@ -132,8 +144,6 @@ extern "C" cuipm_solver *cuipm_create(const cuipm_shape *shape, int max_batch, i
          && cudaMemsetAsync(s->d_sol, 0, sizeof(double) * s->P.sol_stride * max_batch, s->stream) == cudaSuccess
          && cudaStreamSynchronize(s->stream) == cudaSuccess;
     if (!ok) { set_error(std::string("cuipm_create: streams / events / initial clears: ") + cudaGetErrorString(cudaGetLastError())); return fail(); }
-    // default warps per QP: one warp owns one QP unless the stage block is large
-    s->warps = s->P.nmax > 40 ? 4 : 1;
     return s;
 }
 
@@ -143,7 +153,8 @@ extern "C" void cuipm_destroy(cuipm_solver *s)
     cudaSetDevice(s->device);
     if (s->stream) cudaStreamSynchronize(s->stream);
     cudaFree(s->d_sd); cudaFree(s->d_ipool); cudaFree(s->d_qp); cudaFree(s->d_sol); cudaFree(s->d_work);
-    cudaFree(s->d_stat); cudaFree(s->d_info); cudaFree(s->d_seed); cudaFree(s->d_sens); cudaFree(s->d_spill);
+    cudaFree(s->d_stat); cudaFree(s->d_info); cudaFree(s->d_seed); cudaFree(s->d_sens);
+    s->generic.destroy();
     s->fast.destroy();
     if (s->ev0) cudaEventDestroy(s->ev0);
     if (s->ev1) cudaEventDestroy(s->ev1);
@@ -190,12 +201,7 @@ extern "C" float cuipm_last_kernel_ms(const cuipm_solver *s) { return s->last_ms
 
 extern "C" int cuipm_set_tuning(cuipm_solver *s, const char *key, int value)
 {
-    if (!std::strcmp(key, "warps"))
-    {
-        if (value != 1 && value != 2 && value != 4) { set_error("warps must be 1, 2 or 4"); return CUIPM_ERR_INVALID; }
-        s->warps = value;
-        return CUIPM_OK;
-    }
+    if (!std::strcmp(key, "warps")) return s->generic.set_warps(value);
     if (!std::strcmp(key, "pipe"))
     {
         if (value < 1 || value > cuipm_solver::kPipe) { set_error("pipe must be in 1..8"); return CUIPM_ERR_INVALID; }
@@ -214,14 +220,8 @@ extern "C" int cuipm_set_tuning(cuipm_solver *s, const char *key, int value)
     }
     if (!std::strcmp(key, "spill"))
     {
-        // 1 runs the global-scratch variant on a shape that fits in shared memory too; 0 restores the plan's choice
-        if (value != 0 && !s->d_spill)
-        {
-            CK(cudaSetDevice(s->device));
-            CK(cudaMalloc(&s->d_spill, sizeof(double) * spill_doubles(s->P) * (size_t) s->max_batch));
-        }
-        s->spill = s->P.spill || value != 0;
-        return CUIPM_OK;
+        CK(cudaSetDevice(s->device));
+        return s->generic.set_spill(value);
     }
     set_error("unknown tuning key");
     return CUIPM_ERR_INVALID;
@@ -404,10 +404,9 @@ extern "C" int cuipm_sens_device(cuipm_solver *s, int nbatch, const double *d_qp
     a.P = s->P; a.sd = s->d_sd; a.ipool = s->d_ipool; a.qp = d_qp; a.sol = nullptr; a.work = s->d_work; a.info = nullptr;
     a.stat = nullptr; a.o = *opts; a.nbatch = nbatch; a.seed = d_seed; a.sens = d_sens; a.adjoint = adjoint != 0;
     a.redo_list = nullptr; a.redo_count = nullptr;
-    a.spill = s->spill ? s->d_spill : nullptr;
     CK(cudaEventRecord(s->ev0, s->stream));
-    int e = launch_sens(a, s->warps, (void *) s->stream);
-    if (e != 0) { set_error(std::string("kernel launch: ") + cudaGetErrorString((cudaError_t) e)); return CUIPM_ERR_CUDA; }
+    rc = s->generic.sens(a, (void *) s->stream);
+    if (rc != CUIPM_OK) return rc;
     s->last_launches = 1;
     CK(cudaEventRecord(s->ev1, s->stream));
     if (sync)

@@ -4,6 +4,8 @@
 // d_part_cond_qp_expand_sol (external/hpipm/cond/x_part_cond.c:410-866).
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <cstdint>
 #include <string>
 
 #include "cuipm.h"
@@ -26,7 +28,7 @@ struct CtaExec
     }
 };
 
-// GSCR: the scratch of a block that needs more than 227 KB is QP q's slice of a device buffer (gscr, scr_stride doubles per QP)
+// GSCR: the scratch of a block that does not fit in shared memory is QP q's slice of a device buffer (gscr, scr_stride doubles per QP)
 template <int MODE, bool GSCR>
 __global__ void condense_kernel(Plan P, const double *qp, double *qp2, double *tbuf, double *gscr, size_t scr_stride, int nbatch)
 {
@@ -61,7 +63,7 @@ struct cuipm_condenser
     size_t smem_exp = 0;          // ... and of the expansion kernel
     double *d_t = nullptr;        // T_j of the QPs of the last lhs pass (t_stride doubles per QP)
     int t_cap = 0, t_valid = 0;   // QPs the buffer holds / QPs the last lhs pass filled
-    // condensed blocks whose scratch exceeds 227 KB: the scratch of QP q is d_scr + q * scr_stride (grown on demand, like d_t;
+    // condensed blocks whose scratch does not fit in shared memory: the scratch of QP q is d_scr + q * scr_stride (grown on demand, like d_t;
     // calls of one condenser therefore go on one stream, or do not overlap)
     bool gscr = false;
     size_t scr_stride = 0;
@@ -69,36 +71,28 @@ struct cuipm_condenser
     int scr_cap = 0;
 };
 
-#define CKC(call)                                                                                       \
-    do {                                                                                                \
-        cudaError_t e_ = (call);                                                                        \
-        if (e_ != cudaSuccess)                                                                          \
-        {                                                                                               \
-            set_error(std::string(#call) + ": " + cudaGetErrorString(e_));                              \
-            return CUIPM_ERR_CUDA;                                                                      \
-        }                                                                                               \
-    } while (0)
-
 // launches condense_kernel<MODE> with the scratch where the plan needs it
 template <int MODE>
 static int launch_condense(cuipm_condenser *c, int nbatch, const double *d_qp, double *d_qp_cond, double *tbuf, cudaStream_t stream)
 {
     if (!c->gscr)
     {
+        const int rc = set_dynamic_smem((const void *) condense_kernel<MODE, false>, c->smem);
+        if (rc != CUIPM_OK) return rc;
         condense_kernel<MODE, false><<<nbatch, 128, c->smem, stream>>>(c->P, d_qp, d_qp_cond, tbuf, nullptr, 0, nbatch);
-        CKC(cudaGetLastError());
+        CK(cudaGetLastError());
         return CUIPM_OK;
     }
     if (c->scr_cap < nbatch)
     {
-        CKC(cudaStreamSynchronize(stream));
+        CK(cudaStreamSynchronize(stream));
         cudaFree(c->d_scr);
         c->d_scr = nullptr; c->scr_cap = 0;
-        CKC(cudaMalloc(&c->d_scr, sizeof(double) * c->scr_stride * (size_t) nbatch));
+        CK(cudaMalloc(&c->d_scr, sizeof(double) * c->scr_stride * (size_t) nbatch));
         c->scr_cap = nbatch;
     }
     condense_kernel<MODE, true><<<nbatch, 128, 0, stream>>>(c->P, d_qp, d_qp_cond, tbuf, c->d_scr, c->scr_stride, nbatch);
-    CKC(cudaGetLastError());
+    CK(cudaGetLastError());
     return CUIPM_OK;
 }
 
@@ -136,7 +130,16 @@ extern "C" cuipm_condenser *cuipm_condenser_create(const cuipm_shape *shape, int
     c->P = c->hp.plan(c->d_i, c->d_u);
     c->smem = sizeof(double) * (size_t) scratch_doubles(c->P);
     c->smem_exp = c->smem;
-    if (c->smem > 227 * 1024)
+    // the on-chip scratch must fit every kernel that uses it
+    size_t limit = SIZE_MAX;
+    for (const void *k : {(const void *) condense_kernel<COND_ALL, false>, (const void *) condense_kernel<COND_LHS, false>,
+                          (const void *) condense_kernel<COND_RHS, false>, (const void *) expand_kernel})
+    {
+        size_t l = 0;
+        if (smem_limit(k, &l) != CUIPM_OK) { cuipm_condenser_destroy(c); return nullptr; }
+        limit = std::min(limit, l);
+    }
+    if (c->smem > limit)
     {
         // the scratch goes to a device buffer, one slice per QP; the expansion needs only its first 4 nxmax doubles
         c->gscr = true;
@@ -144,10 +147,6 @@ extern "C" cuipm_condenser *cuipm_condenser_create(const cuipm_shape *shape, int
         c->smem = 0;
         c->smem_exp = sizeof(double) * (size_t) expand_scratch_doubles(c->P);
     }
-    cudaFuncSetAttribute(condense_kernel<COND_ALL, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem);
-    cudaFuncSetAttribute(condense_kernel<COND_LHS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem);
-    cudaFuncSetAttribute(condense_kernel<COND_RHS, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem);
-    cudaFuncSetAttribute(expand_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c->smem_exp);
     return c;
 }
 
@@ -157,9 +156,9 @@ extern "C" int cuipm_condense_device(cuipm_condenser *c, int nbatch, const doubl
 {
     if (!c || nbatch < 0 || !d_qp || !d_qp_cond) { set_error("cuipm_condense_device: bad arguments"); return CUIPM_ERR_INVALID; }
     if (nbatch == 0) return CUIPM_OK;
-    CKC(cudaSetDevice(c->device));
+    CK(cudaSetDevice(c->device));
     // the masks of a fresh record are 1 and untouched entries of d / Z / z are 0 in the reference's layout: clear, then fill
-    CKC(cudaMemsetAsync(d_qp_cond, 0, sizeof(double) * c->hp.lc->qp_stride * (size_t) nbatch, (cudaStream_t) stream));
+    CK(cudaMemsetAsync(d_qp_cond, 0, sizeof(double) * c->hp.lc->qp_stride * (size_t) nbatch, (cudaStream_t) stream));
     return launch_condense<COND_ALL>(c, nbatch, d_qp, d_qp_cond, nullptr, (cudaStream_t) stream);
 }
 
@@ -171,16 +170,16 @@ extern "C" int cuipm_condense_lhs_device(cuipm_condenser *c, int nbatch, const d
 {
     if (!c || nbatch < 0 || !d_qp || !d_qp_cond) { set_error("cuipm_condense_lhs_device: bad arguments"); return CUIPM_ERR_INVALID; }
     if (nbatch == 0) return CUIPM_OK;
-    CKC(cudaSetDevice(c->device));
+    CK(cudaSetDevice(c->device));
     if (c->t_cap < nbatch)
     {
-        CKC(cudaStreamSynchronize((cudaStream_t) stream));
+        CK(cudaStreamSynchronize((cudaStream_t) stream));
         cudaFree(c->d_t);
         c->d_t = nullptr; c->t_cap = 0; c->t_valid = 0;
-        CKC(cudaMalloc(&c->d_t, sizeof(double) * (size_t) c->P.t_stride * (size_t) nbatch));
+        CK(cudaMalloc(&c->d_t, sizeof(double) * (size_t) c->P.t_stride * (size_t) nbatch));
         c->t_cap = nbatch;
     }
-    CKC(cudaMemsetAsync(d_qp_cond, 0, sizeof(double) * c->hp.lc->qp_stride * (size_t) nbatch, (cudaStream_t) stream));
+    CK(cudaMemsetAsync(d_qp_cond, 0, sizeof(double) * c->hp.lc->qp_stride * (size_t) nbatch, (cudaStream_t) stream));
     const int rc = launch_condense<COND_LHS>(c, nbatch, d_qp, d_qp_cond, c->d_t, (cudaStream_t) stream);
     if (rc != CUIPM_OK) return rc;
     c->t_valid = nbatch;
@@ -192,7 +191,7 @@ extern "C" int cuipm_condense_rhs_device(cuipm_condenser *c, int nbatch, const d
     if (!c || nbatch < 0 || !d_qp || !d_qp_cond) { set_error("cuipm_condense_rhs_device: bad arguments"); return CUIPM_ERR_INVALID; }
     if (nbatch > c->t_valid) { set_error("cuipm_condense_rhs_device: no lhs pass for this many QPs (call cuipm_condense_lhs_device first)"); return CUIPM_ERR_INVALID; }
     if (nbatch == 0) return CUIPM_OK;
-    CKC(cudaSetDevice(c->device));
+    CK(cudaSetDevice(c->device));
     return launch_condense<COND_RHS>(c, nbatch, d_qp, d_qp_cond, c->d_t, (cudaStream_t) stream);
 }
 
@@ -200,9 +199,11 @@ extern "C" int cuipm_expand_device(cuipm_condenser *c, int nbatch, const double 
 {
     if (!c || nbatch < 0 || !d_qp || !d_sol_cond || !d_sol) { set_error("cuipm_expand_device: bad arguments"); return CUIPM_ERR_INVALID; }
     if (nbatch == 0) return CUIPM_OK;
-    CKC(cudaSetDevice(c->device));
-    CKC(cudaMemsetAsync(d_sol, 0, sizeof(double) * c->hp.lo->sol_stride * (size_t) nbatch, (cudaStream_t) stream));
+    CK(cudaSetDevice(c->device));
+    CK(cudaMemsetAsync(d_sol, 0, sizeof(double) * c->hp.lo->sol_stride * (size_t) nbatch, (cudaStream_t) stream));
+    const int rc = set_dynamic_smem((const void *) expand_kernel, c->smem_exp);
+    if (rc != CUIPM_OK) return rc;
     expand_kernel<<<nbatch, 128, c->smem_exp, (cudaStream_t) stream>>>(c->P, d_qp, d_sol_cond, d_sol, nbatch);
-    CKC(cudaGetLastError());
+    CK(cudaGetLastError());
     return CUIPM_OK;
 }

@@ -10,7 +10,7 @@
 //
 // Data parallelism inside a QP: every phase is "thread t handles elements t, t+NT, ... of an output array" (column-major, so
 // consecutive threads touch consecutive addresses of the records); the small operands T, c, Q T live in the CTA's scratch
-// (shared memory, or the QP's slice of a device buffer where the blocks need more than 227 KB: cuipm_condense.cu).
+// (shared memory, or the QP's slice of a device buffer where the blocks need more than a block may have: cuipm_condense.cu).
 #ifndef CUIPM_CONDENSE_CORE_H_
 #define CUIPM_CONDENSE_CORE_H_
 

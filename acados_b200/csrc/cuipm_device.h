@@ -43,11 +43,9 @@ struct ProbDesc
     int mid_nx, mid_nu;                                    // (nx, nu) shared by stages 1..N-1 and nx of stage N, or 0,0 if not uniform
     unsigned w_lq;                                         // work record: nmax x (nbgmax + nxmax) scratch of the LQ refactorisation
     unsigned w_bkp;                                        // work record: lam, t of the iterate of the last factorisation, in a record of the solution layout
-    int spill;                                             // 1: the stage-block buffers (sm_M, sm_A, sm_AL, sm_C) do not fit in shared memory
-                                                           //    next to sm_V; the generic kernel keeps them in a per-QP slice of a device
-                                                           //    scratch buffer (spill_doubles(P) doubles per QP) instead
     size_t qp_stride, sol_stride, work_stride;
-    // shared-memory carve (doubles)
+    // shared-memory carve (doubles).  sm_A is always 0 (the sweeps stream those matrices), but the generic kernel's address sums
+    // keep it: without the term ptxas allocates the kernel's registers worse (more local-memory spills in the sweeps)
     int sm_M, sm_A, sm_AL, sm_C, sm_V;
     int sm_total;
 };
@@ -141,10 +139,30 @@ constexpr bool fast_packed(int nx, int nu) { return nx + nu <= 32; }
 // status value the throughput kernel leaves in cuipm_info::status of a QP it hands back (never seen by callers)
 #define CUIPM_FAST_REDO 100
 
-// launches the solve kernel with `warps` warps per QP on `stream`; returns cudaError_t as int
-int launch_solve(const LaunchArgs &a, int warps, void *stream);
-// launches the sensitivity kernel (one substitution with the factorisation the last solve left in the work records)
-int launch_sens(const LaunchArgs &a, int warps, void *stream);
+struct GenericInstance;   // compiled instance of the generic kernel (cuipm_kernel.cu)
+
+// The generic kernel's host side for one solver (cuipm_kernel.cu): warps per QP, stage-block buffers on chip or in a device scratch
+// buffer (the global-scratch variant), that buffer, and the launches.
+struct GenericPath
+{
+    int warps = 1;                        // tuning key "warps": warps per QP (1, 2 or 4)
+    int spill = 0;                        // the global-scratch variant runs: the shape needs it, or tuning key "spill"
+    int spill_needed = 0;                 // the stage-block buffers do not fit in shared memory next to the vector area
+    int sms = 1;                          // SMs of the solver's device
+    size_t scratch_bytes = 0;             // scratch for max_batch QPs, spill_doubles(P) doubles each
+    double *d_spill = nullptr;            // the scratch (null until the variant is used)
+
+    // Picks the default warps per QP, decides on chip or global scratch against the limit of `device` (the current device) and
+    // allocates the scratch if needed.  This and the calls below return CUIPM_OK or an error code with the message set.
+    int create(const ProbDesc &P, int max_batch, int device);
+    // the solve kernel over batch `a` (QPs lo .. lo + a.nbatch - 1 of the solver's buffers; a.redo_list / a.redo_count, if set: the
+    // QPs the throughput kernel handed back), and the sensitivity kernel (one substitution with the last solve's factorisation)
+    int solve(LaunchArgs a, size_t lo, void *stream) const;
+    int sens(LaunchArgs a, void *stream) const;
+    int set_warps(int value);   // tuning key "warps": 1, 2 or 4
+    int set_spill(int value);   // tuning key "spill": 1 runs the global-scratch variant on a shape that fits too, 0 restores create's choice
+    void destroy();
+};
 
 struct FastInstance;   // compiled instance of the throughput kernel (cuipm_fast.cu)
 

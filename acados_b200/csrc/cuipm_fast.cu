@@ -205,16 +205,6 @@ static const FastInstance kInstances[] = {
 #undef X
 };
 
-#define CKF(what, call)                                                                                 \
-    do {                                                                                                \
-        cudaError_t e_ = (call);                                                                        \
-        if (e_ != cudaSuccess)                                                                          \
-        {                                                                                               \
-            set_error(std::string(what) + ": " + cudaGetErrorString(e_));                               \
-            return CUIPM_ERR_CUDA;                                                                      \
-        }                                                                                               \
-    } while (0)
-
 // The dynamic shared memory attribute belongs to the kernel, not to a solver: solvers of other shapes may launch the same
 // instance with more, so it is set before every launch.  The CTAs of one SM together need most of its shared memory: ask for
 // the largest carve-out (the default heuristic sized it for a single CTA, which left one warp per SM resident).
@@ -233,25 +223,32 @@ int FastPath::create(const std::vector<StageDesc> &sd, const std::vector<int> &i
         if (i.nx == F.s1.nx && i.nu == F.s1.nu) in = &i;
     if (!in) return CUIPM_OK;
     smem = in->layout(F);
-    if (smem > 226 * 1024) return CUIPM_OK;
+    for (FastKernel k : in->kernel)
+    {
+        size_t limit = 0;
+        const int rc = smem_limit((const void *) k, &limit);
+        if (rc != CUIPM_OK) return rc;
+        if (smem > limit) return CUIPM_OK;
+    }
     inst = in;
     nslot = nslot_;
     const size_t nb = (size_t) max_batch;
-    CKF("cudaMalloc", cudaMalloc(&redo_list, sizeof(int) * nb));
-    CKF("cudaMalloc", cudaMalloc(&ctr, sizeof(int) * 2 * nslot));
-    CKF("cudaMemset", cudaMemset(ctr, 0, sizeof(int) * 2 * nslot));
-    CKF("cudaMalloc", cudaMalloc(&qpk, sizeof(double) * F.qpk_stride * nb));
-    CKF("cudaMemset", cudaMemset(qpk, 0, sizeof(double) * F.qpk_stride * nb));
-    CKF("cudaMalloc", cudaMalloc(&rr_state, sizeof(double) * 12 * nb));
-    CKF("cudaMalloc", cudaMalloc(&rr_ring, sizeof(int) * CUIPM_RR_RINGS * nb));
-    CKF("cudaMalloc", cudaMalloc(&rr_ctr, sizeof(int) * CUIPM_RR_CTR * nslot));
+    CK(cudaMalloc(&redo_list, sizeof(int) * nb));
+    CK(cudaMalloc(&ctr, sizeof(int) * 2 * nslot));
+    CK(cudaMemset(ctr, 0, sizeof(int) * 2 * nslot));
+    CK(cudaMalloc(&qpk, sizeof(double) * F.qpk_stride * nb));
+    CK(cudaMemset(qpk, 0, sizeof(double) * F.qpk_stride * nb));
+    CK(cudaMalloc(&rr_state, sizeof(double) * 12 * nb));
+    CK(cudaMalloc(&rr_ring, sizeof(int) * CUIPM_RR_RINGS * nb));
+    CK(cudaMalloc(&rr_ctr, sizeof(int) * CUIPM_RR_CTR * nslot));
     // residency with this solver's shared memory, per mode (the three kernels need different numbers of registers)
-    CKF("cudaDeviceGetAttribute", cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
     for (int m = 0; m < 3; m++)
     {
         int nblk = 0;
-        CKF("cudaFuncSetAttribute", set_smem(inst->kernel[m], smem));
-        CKF("cudaOccupancyMaxActiveBlocksPerMultiprocessor", cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, inst->kernel[m], 32, smem));
+        const cudaError_t e = set_smem(inst->kernel[m], smem);
+        if (e != cudaSuccess) return cuda_error("shared memory attributes of the throughput kernel", e);
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, inst->kernel[m], 32, smem));
         ctas[m] = (nblk > 0 ? nblk : 1) * sms;
         if (m == 0) ring_qps = nblk * sms * inst->qpw;
     }
@@ -280,9 +277,10 @@ int FastPath::enqueue(LaunchArgs &a, size_t lo, int slot, void *stream_, int *la
     f.nbatch = a.nbatch; f.ipool = a.ipool; f.qp = a.qp; f.sol = a.sol; f.work = a.work; f.info = a.info; f.stat = a.stat; f.o = a.o;
     f.qpk = qpk + F.qpk_stride * lo;
     f.redo_list = redo_list + lo; f.redo_count = ctr + 2 * slot; f.next_qp = f.redo_count + 1;
-    CKF("cudaMemsetAsync", cudaMemsetAsync(f.redo_count, 0, 2 * sizeof(int), stream));
+    CK(cudaMemsetAsync(f.redo_count, 0, 2 * sizeof(int), stream));
     cuipm_repack_kernel<<<f.nbatch < sms * 8 ? f.nbatch : sms * 8, 256, 0, stream>>>(f, a.sd);      // eight CTAs per SM, grid-stride over the batch
-    CKF("kernel launch (repack)", cudaGetLastError());
+    const cudaError_t er = cudaGetLastError();
+    if (er != cudaSuccess) return cuda_error("kernel launch (repack)", er);
     (*launches)++;
     if (ev_repacked) cudaEventRecord((cudaEvent_t) ev_repacked, stream);
     // iteration-sliced scheduling pays when the batch is more than one wave of resident QPs and not many; small batches keep the
@@ -291,15 +289,15 @@ int FastPath::enqueue(LaunchArgs &a, size_t lo, int slot, void *stream_, int *la
     if (rr && (rr > 1 || (ring_qps > 0 && a.nbatch > ring_qps)))
     {
         f.rr_state = rr_state + 12 * lo; f.rr_ring = rr_ring + CUIPM_RR_RINGS * lo; f.rr_ctr = rr_ctr + CUIPM_RR_CTR * slot;
-        CKF("cudaMemsetAsync", cudaMemsetAsync(f.rr_ring, 0xff, sizeof(int) * CUIPM_RR_RINGS * (size_t) a.nbatch, stream));
-        CKF("cudaMemsetAsync", cudaMemsetAsync(f.rr_ctr, 0, CUIPM_RR_CTR * sizeof(int), stream));
+        CK(cudaMemsetAsync(f.rr_ring, 0xff, sizeof(int) * CUIPM_RR_RINGS * (size_t) a.nbatch, stream));
+        CK(cudaMemsetAsync(f.rr_ctr, 0, CUIPM_RR_CTR * sizeof(int), stream));
         e = launch(*this, 1, f, stream);
         if (e == cudaSuccess) { (*launches)++; e = launch(*this, 2, f, stream); }
     }
     else
         e = launch(*this, 0, f, stream);
     if (ev_done) cudaEventRecord((cudaEvent_t) ev_done, stream);
-    CKF("kernel launch (throughput kernel)", e);
+    if (e != cudaSuccess) return cuda_error("kernel launch (throughput kernel)", e);
     (*launches)++;
     a.redo_list = f.redo_list;
     a.redo_count = f.redo_count;

@@ -2,6 +2,7 @@
 #ifndef CUIPM_INTERNAL_H_
 #define CUIPM_INTERNAL_H_
 
+#include <cstddef>
 #include <string>
 
 #include "cuipm.h"
@@ -10,6 +11,17 @@ namespace cuipm {
 void set_error(const std::string &msg);
 // CUIPM_OK if the option values are within what the device path implements, else CUIPM_ERR_INVALID (+ message)
 int opts_check(const cuipm_opts *o);
+// Dynamic shared memory (bytes) `kernel` may request per block on the current device: the device's opt-in limit less the
+// kernel's static shared memory.  Returns CUIPM_OK or CUIPM_ERR_CUDA (+ message).
+int smem_limit(const void *kernel, size_t *bytes);
+// Sets the dynamic shared memory `kernel` may be launched with.  The attribute belongs to the kernel, not to a solver: objects of
+// other shapes in the process may launch the same kernel with more or less, so it is set before every launch.
+int set_dynamic_smem(const void *kernel, size_t bytes);
+// Sets the message "<what>: <CUDA error string of err (a cudaError_t)>" and returns CUIPM_ERR_CUDA.
+int cuda_error(const std::string &what, int err);
 }  // namespace cuipm
+
+// CUDA runtime call in a function that returns a cuipm status: on failure, the message names the call
+#define CK(call) do { const cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuipm::cuda_error(#call, (int) e_); } while (0)
 
 #endif

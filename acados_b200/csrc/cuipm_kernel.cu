@@ -10,9 +10,13 @@
 // This file is the generic path: any per-stage dimensions, box / general / soft constraints, masks.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
+#include <cstdint>
+#include <string>
 
 #include "cuipm_device.h"
+#include "cuipm_internal.h"
 
 namespace cuipm {
 
@@ -27,8 +31,8 @@ __device__ __forceinline__ int ev(int n) { return (n + 1) & ~1; }
 // dynamic shared memory is reached through the extern array below, so that every on-chip access compiles to LDS/STS
 // with 32-bit addressing instead of generic loads.
 //
-// Global-scratch variant (Ker<..., SPILL = true>, for shapes whose buffers exceed 227 KB of shared memory): the stage-block
-// buffers SM_, SA_, SAL_, SC_ are this QP's slice of a device scratch buffer (Ctx::spx), the vector area SV_ and the context
+// Global-scratch variant (Ker<..., SPILL = true>, for shapes whose buffers exceed the shared memory a block may have): the
+// stage-block buffers SM_, SAL_, SC_ are this QP's slice of a device scratch buffer (Ctx::spx), the vector area SV_ and the context
 // stay on chip.  The sweeps perform the same arithmetic in the same order on the same operands; only the copies into those
 // buffers change, from LDGSTS (cp.async needs a shared destination) to plain loads and stores (cpb8 / cpvb).  __syncthreads /
 // __syncwarp order global memory among the CTA's threads as they order shared memory.
@@ -58,7 +62,6 @@ extern __shared__ __align__(16) double g_smem[];
 // SPILL is the template parameter of Ker (and of the kernels): a compile-time constant, so the on-chip variant's addresses
 // are those of the plain extern array
 #define SM_ (SPILL ? CX.spx : g_smem)
-#define SA_ (SM_ + CX.P.sm_M)
 #define SAL_ (SM_ + CX.P.sm_M + CX.P.sm_A)
 #define SC_ (SM_ + CX.P.sm_M + CX.P.sm_A + CX.P.sm_AL)
 #define SV_ (SPILL ? g_smem : g_smem + CX.P.sm_M + CX.P.sm_A + CX.P.sm_AL + CX.P.sm_C)
@@ -2007,15 +2010,9 @@ struct Ker
 
 };
 
-#ifndef CUIPM_MINB
-#define CUIPM_MINB 16
-#endif
-// resident CTAs per SM the register allocation is bounded for: the on-chip variant 16 / 8 / 4 (W = 1 / 2 / 4); the global-scratch
-// variant 1, so that its register allocation is unconstrained (no local-memory spills): its shapes are too large for more
-// than a few CTAs per SM to help, and they run from L2 anyway
-#define CUIPM_MIN_CTAS(W, SPILL) ((SPILL) ? 1 : ((W) == 1 ? CUIPM_MINB : ((W) == 2 ? 8 : 4)))
-template <int W, int SNX, int SNU, bool SPILL>
-__global__ void __launch_bounds__(32 * W, CUIPM_MIN_CTAS(W, SPILL)) cuipm_solve_kernel(const LaunchArgs a)
+// MINB: resident CTAs per SM the register allocation is bounded for (CUIPM_GENERIC_INSTANCES below)
+template <int W, int SNX, int SNU, bool SPILL, int MINB>
+__global__ void __launch_bounds__(32 * W, MINB) cuipm_solve_kernel(const LaunchArgs a)
 {
     if (threadIdx.x == 0)
     {
@@ -2045,8 +2042,8 @@ __global__ void __launch_bounds__(32 * W, CUIPM_MIN_CTAS(W, SPILL)) cuipm_solve_
     }
 }
 
-template <int W, bool SPILL>
-__global__ void __launch_bounds__(32 * W, CUIPM_MIN_CTAS(W, SPILL)) cuipm_sens_kernel(const LaunchArgs a)
+template <int W, bool SPILL, int MINB>
+__global__ void __launch_bounds__(32 * W, MINB) cuipm_sens_kernel(const LaunchArgs a)
 {
     if (threadIdx.x == 0)
     {
@@ -2075,67 +2072,116 @@ __global__ void __launch_bounds__(32 * W, CUIPM_MIN_CTAS(W, SPILL)) cuipm_sens_k
 
 }  // namespace
 
-// dynamic shared memory (bytes) the kernel needs for P: every buffer, or the vector area alone in the global-scratch variant
-static size_t smem_bytes(const LaunchArgs &a) { return sizeof(double) * (size_t) (a.spill ? a.P.sm_V : a.P.sm_total); }
+// ---- host side of the generic path (GenericPath, cuipm_device.h) -------------------------------------------------------
 
-template <int W, int SNX, int SNU, bool SPILL = false>
-static cudaError_t launch_one(const LaunchArgs &a, size_t smem, cudaStream_t stream)
+// the compiled instances: warps per QP, interior (nx, nu) of the specialised sweeps (0, 0: any shape, these have a sensitivity kernel
+// too), global-scratch variant, and the resident CTAs per SM the registers are bounded for: 1 in the global-scratch variant, so that
+// it does not spill (its shapes gain nothing from more CTAs per SM, and they run from L2 anyway)
+#define CUIPM_GENERIC_INSTANCES(X)                                                              \
+    X(1, 21, 3, false, 16) X(1, 8, 3, false, 16) X(1, 4, 1, false, 16) X(1, 12, 4, false, 16) \
+    X(1, 0, 0, false, 16) X(2, 0, 0, false, 8) X(4, 0, 0, false, 4)                           \
+    X(1, 0, 0, true, 1) X(2, 0, 0, true, 1) X(4, 0, 0, true, 1)
+
+typedef void (*GenericKernel)(LaunchArgs);
+
+struct GenericInstance
 {
-    cudaError_t err = cudaFuncSetAttribute(cuipm_solve_kernel<W, SNX, SNU, SPILL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-    if (err != cudaSuccess) return err;
-    // behind the throughput kernel only a few QPs are left: a small grid whose blocks walk the hand-back list
-    const int grid = a.redo_list ? (a.nbatch < 1184 ? a.nbatch : 1184) : a.nbatch;
-    cuipm_solve_kernel<W, SNX, SNU, SPILL><<<grid, 32 * W, smem, stream>>>(a);
-    return cudaGetLastError();
+    int warps, snx, snu, spill;
+    GenericKernel solve, sens;   // sens: null for a specialisation
+};
+
+template <int W, int SNX, bool SPILL, int MINB>
+static GenericKernel sens_kernel() { if constexpr (SNX == 0) return cuipm_sens_kernel<W, SPILL, MINB>; else return nullptr; }
+
+static const GenericInstance kGeneric[] = {
+#define X(W_, SNX_, SNU_, SPILL_, MB_) {W_, SNX_, SNU_, SPILL_, cuipm_solve_kernel<W_, SNX_, SNU_, SPILL_, MB_>, sens_kernel<W_, SNX_, SPILL_, MB_>()},
+    CUIPM_GENERIC_INSTANCES(X)
+#undef X
+};
+
+// the instance for `warps` and the variant: the specialisation for interior stages (nx, nu) if there is one, else the one for any shape
+static const GenericInstance &instance_for(int warps, int spill, int nx, int nu)
+{
+    const GenericInstance *any = &kGeneric[0];
+    for (const GenericInstance &i : kGeneric)
+        if (i.warps == warps && i.spill == spill)
+        {
+            if (i.snx == nx && i.snu == nu) return i;
+            if (i.snx == 0) any = &i;
+        }
+    return *any;
 }
 
-// (nx, nu) pairs with a compile-time specialisation of the interior stages (BASELINE.json configs 1-4); any other
-// shape runs the generic path.  With a scratch buffer (a.spill): the global-scratch variant, generic dimensions only.
-int launch_solve(const LaunchArgs &a, int warps, void *stream_)
+// dynamic shared memory (bytes) of a launch for P: every buffer on chip, or the vector area alone in the global-scratch variant
+static size_t smem_bytes(const ProbDesc &P, bool spill) { return sizeof(double) * (size_t) (spill ? P.sm_V : P.sm_total); }
+
+static int launch(GenericKernel k, const LaunchArgs &a, int grid, int warps, void *stream)
 {
-    cudaStream_t stream = (cudaStream_t) stream_;
-    const size_t smem = smem_bytes(a);
-    if (a.spill)
+    const size_t smem = smem_bytes(a.P, a.spill != nullptr);
+    const int rc = set_dynamic_smem((const void *) k, smem);
+    if (rc != CUIPM_OK) return rc;
+    k<<<grid, 32 * warps, smem, (cudaStream_t) stream>>>(a);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? CUIPM_OK : cuda_error("kernel launch", e);
+}
+
+int GenericPath::create(const ProbDesc &P, int max_batch, int device)
+{
+    warps = P.nmax > 40 ? 4 : 1;   // one warp owns one QP unless the stage block is large
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+    // the dynamic shared memory every instance of a variant (0 on chip, 1 global scratch) may request: the choice holds for any "warps"
+    size_t lim[2] = {SIZE_MAX, SIZE_MAX};
+    for (const GenericInstance &i : kGeneric)
+        for (GenericKernel k : {i.solve, i.sens})
+        {
+            size_t l = 0;
+            if (!k) continue;   // the specialisations have no sensitivity kernel
+            if (smem_limit((const void *) k, &l) != CUIPM_OK) return CUIPM_ERR_CUDA;
+            lim[i.spill] = std::min(lim[i.spill], l);
+        }
+    // shapes whose buffers do not fit keep the stage-block buffers in a device scratch buffer, the vector area on chip
+    spill_needed = spill = smem_bytes(P, false) > lim[0];
+    if (spill && smem_bytes(P, true) > lim[1])
     {
-        if (warps <= 1) return (int) launch_one<1, 0, 0, true>(a, smem, stream);
-        if (warps == 2) return (int) launch_one<2, 0, 0, true>(a, smem, stream);
-        return (int) launch_one<4, 0, 0, true>(a, smem, stream);
+        set_error("stage dimensions need more than the " + std::to_string(lim[1]) + " bytes of shared memory a block may have for the "
+                  "solver's vectors alone");
+        return CUIPM_ERR_TOO_LARGE;
     }
-    if (warps <= 1)
-    {
-        const int nx = a.P.mid_nx, nu = a.P.mid_nu;
-        if (nx == 21 && nu == 3) return (int) launch_one<1, 21, 3>(a, smem, stream);
-        if (nx == 8 && nu == 3) return (int) launch_one<1, 8, 3>(a, smem, stream);
-        if (nx == 4 && nu == 1) return (int) launch_one<1, 4, 1>(a, smem, stream);
-        if (nx == 12 && nu == 4) return (int) launch_one<1, 12, 4>(a, smem, stream);
-        return (int) launch_one<1, 0, 0>(a, smem, stream);
-    }
-    if (warps == 2) return (int) launch_one<2, 0, 0>(a, smem, stream);
-    return (int) launch_one<4, 0, 0>(a, smem, stream);
+    // a separate buffer, not part of the work record: the getters, the sensitivities and the hand-back path read that layout
+    scratch_bytes = sizeof(double) * spill_doubles(P) * (size_t) max_batch;
+    if (spill) CK(cudaMalloc(&d_spill, scratch_bytes));
+    return CUIPM_OK;
 }
 
-template <int W, bool SPILL>
-static cudaError_t launch_sens_one(const LaunchArgs &a, size_t smem, cudaStream_t stream)
+int GenericPath::solve(LaunchArgs a, size_t lo, void *stream) const
 {
-    cudaError_t err = cudaFuncSetAttribute(cuipm_sens_kernel<W, SPILL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-    if (err != cudaSuccess) return err;
-    cuipm_sens_kernel<W, SPILL><<<a.nbatch, 32 * W, smem, stream>>>(a);
-    return cudaGetLastError();
+    // by QP, not by CTA: the chunks of a host solve run concurrently, each with its own part of the scratch
+    a.spill = spill ? d_spill + spill_doubles(a.P) * lo : nullptr;
+    // behind the throughput kernel only a few QPs are left: a small grid (eight CTAs per SM) whose blocks walk the hand-back list
+    const int grid = a.redo_list ? std::min(a.nbatch, 8 * sms) : a.nbatch;
+    return launch(instance_for(warps, spill, a.P.mid_nx, a.P.mid_nu).solve, a, grid, warps, stream);
 }
 
-template <bool SPILL>
-static cudaError_t launch_sens_w(const LaunchArgs &a, int warps, size_t smem, cudaStream_t stream)
+int GenericPath::sens(LaunchArgs a, void *stream) const
 {
-    if (warps <= 1) return launch_sens_one<1, SPILL>(a, smem, stream);
-    if (warps == 2) return launch_sens_one<2, SPILL>(a, smem, stream);
-    return launch_sens_one<4, SPILL>(a, smem, stream);
+    a.spill = spill ? d_spill : nullptr;
+    return launch(instance_for(warps, spill, 0, 0).sens, a, a.nbatch, warps, stream);
 }
 
-int launch_sens(const LaunchArgs &a, int warps, void *stream_)
+int GenericPath::set_warps(int value)
 {
-    cudaStream_t stream = (cudaStream_t) stream_;
-    const size_t smem = smem_bytes(a);
-    return (int) (a.spill ? launch_sens_w<true>(a, warps, smem, stream) : launch_sens_w<false>(a, warps, smem, stream));
+    if (value != 1 && value != 2 && value != 4) { set_error("warps must be 1, 2 or 4"); return CUIPM_ERR_INVALID; }
+    warps = value;
+    return CUIPM_OK;
 }
+
+int GenericPath::set_spill(int value)
+{
+    if (value != 0 && !d_spill) CK(cudaMalloc(&d_spill, scratch_bytes));
+    spill = spill_needed || value != 0;
+    return CUIPM_OK;
+}
+
+void GenericPath::destroy() { cudaFree(d_spill); }
 
 }  // namespace cuipm

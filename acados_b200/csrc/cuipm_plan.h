@@ -111,15 +111,8 @@ inline int build_plan(const cuipm_shape *sh, const cuipm_layout *l, std::vector<
         const int v_init = nvs + nc + e(P.ngmax);
         P.sm_V = std::max(std::max(std::max(v_res, v_fwd), std::max(v_fact, v_slv)), v_init) + 8;
     }
+    // whether this fits in shared memory is the device's question (GenericPath::create)
     P.sm_total = P.sm_M + P.sm_A + P.sm_AL + P.sm_C + P.sm_V;
-    // Shapes whose buffers exceed the 227 KB of shared memory a block may have run the generic kernel's global-scratch
-    // variant: the stage-block buffers move to a device scratch buffer, the vector area stays on chip.
-    P.spill = sizeof(double) * (size_t) P.sm_total > 227 * 1024;
-    if (P.spill && sizeof(double) * (size_t) P.sm_V > 227 * 1024)
-    {
-        err = "stage dimensions need more than 227 KB of shared memory for the solver's vectors alone";
-        return CUIPM_ERR_TOO_LARGE;
-    }
     return CUIPM_OK;
 }
 

@@ -186,16 +186,6 @@ struct cuipm_reducer
     cuipm_shape red{};
 };
 
-#define CKR(call)                                                                                       \
-    do {                                                                                                \
-        cudaError_t e_ = (call);                                                                        \
-        if (e_ != cudaSuccess)                                                                          \
-        {                                                                                               \
-            set_error(std::string(#call) + ": " + cudaGetErrorString(e_));                              \
-            return CUIPM_ERR_CUDA;                                                                      \
-        }                                                                                               \
-    } while (0)
-
 extern "C" void cuipm_reducer_destroy(cuipm_reducer *r)
 {
     if (!r) return;
@@ -308,9 +298,9 @@ extern "C" int cuipm_reduce_device(cuipm_reducer *r, int nbatch, const double *d
 {
     if (!r || nbatch < 0 || !d_qp_full || !d_qp_red) { set_error("cuipm_reduce_device: bad arguments"); return CUIPM_ERR_INVALID; }
     if (nbatch == 0) return CUIPM_OK;
-    CKR(cudaSetDevice(r->device));
+    CK(cudaSetDevice(r->device));
     reduce_kernel<<<nbatch, 128, sizeof(double) * (r->D.ne + 2), (cudaStream_t) stream>>>(r->D, d_qp_full, d_qp_red, nbatch);
-    CKR(cudaGetLastError());
+    CK(cudaGetLastError());
     return CUIPM_OK;
 }
 
@@ -319,9 +309,9 @@ extern "C" int cuipm_restore_device(cuipm_reducer *r, int nbatch, const double *
 {
     if (!r || nbatch < 0 || !d_qp_full || !d_sol_red || !d_sol_full) { set_error("cuipm_restore_device: bad arguments"); return CUIPM_ERR_INVALID; }
     if (nbatch == 0) return CUIPM_OK;
-    CKR(cudaSetDevice(r->device));
+    CK(cudaSetDevice(r->device));
     const size_t sm = sizeof(double) * (r->D.n_f + r->D.nb_f + r->D.ng + 4);
     restore_kernel<<<nbatch, 128, sm, (cudaStream_t) stream>>>(r->D, d_qp_full, d_sol_red, d_sol_full, nbatch, lam_min, t_min);
-    CKR(cudaGetLastError());
+    CK(cudaGetLastError());
     return CUIPM_OK;
 }

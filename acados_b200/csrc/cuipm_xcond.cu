@@ -27,15 +27,6 @@ struct cuipm_xcond
     int lhs_valid = 0;
 };
 
-#define CKX(call)                                                                                       \
-    do {                                                                                                \
-        cudaError_t e_ = (call);                                                                        \
-        if (e_ != cudaSuccess)                                                                          \
-        {                                                                                               \
-            set_error(std::string(#call) + ": " + cudaGetErrorString(e_));                              \
-            return CUIPM_ERR_CUDA;                                                                      \
-        }                                                                                               \
-    } while (0)
 #define RCX(call) do { int rc_ = (call); if (rc_ != CUIPM_OK) return rc_; } while (0)
 
 extern "C" void cuipm_xcond_destroy(cuipm_xcond *x)
@@ -104,9 +95,9 @@ static int chain(cuipm_xcond *x, int mode, int nbatch, const double *qp_full, do
     if (mode != 1 && opts->warm_start >= 2) { set_error("cuipm_xcond: warm starts (warm_start >= 2) are not carried through the chain"); return CUIPM_ERR_INVALID; }
     if (mode == 2 && x->cond && x->lhs_valid < nbatch) { set_error("cuipm_xcond_condense_rhs_and_solve_host: call cuipm_xcond_condense_lhs_host first"); return CUIPM_ERR_INVALID; }
     if (nbatch == 0) return CUIPM_OK;
-    CKX(cudaSetDevice(x->device));
+    CK(cudaSetDevice(x->device));
     cudaStream_t st = (cudaStream_t) cuipm_stream(x->solver);
-    CKX(cudaMemcpyAsync(x->d_full, qp_full, sizeof(double) * x->lf->qp_stride * (size_t) nbatch, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(x->d_full, qp_full, sizeof(double) * x->lf->qp_stride * (size_t) nbatch, cudaMemcpyHostToDevice, st));
     RCX(cuipm_reduce_device(x->red, nbatch, x->d_full, x->d_red, st));
     const double *d_qp = x->d_red;
     if (x->cond)
@@ -116,7 +107,7 @@ static int chain(cuipm_xcond *x, int mode, int nbatch, const double *qp_full, do
         if (mode != 2) x->lhs_valid = nbatch;
         d_qp = x->d_cond;
     }
-    if (mode == 1) { CKX(cudaStreamSynchronize(st)); return CUIPM_OK; }
+    if (mode == 1) { CK(cudaStreamSynchronize(st)); return CUIPM_OK; }
     RCX(cuipm_solve_device(x->solver, nbatch, d_qp, x->d_sol, x->d_info, nullptr, opts, 0));
     const double *d_sr = x->d_sol;
     if (x->cond)
@@ -125,9 +116,9 @@ static int chain(cuipm_xcond *x, int mode, int nbatch, const double *qp_full, do
         d_sr = x->d_sol_red;
     }
     RCX(cuipm_restore_device(x->red, nbatch, x->d_full, d_sr, x->d_sol_full, opts->lam_min, opts->t_min, st));
-    CKX(cudaMemcpyAsync(sol_full, x->d_sol_full, sizeof(double) * x->lf->sol_stride * (size_t) nbatch, cudaMemcpyDeviceToHost, st));
-    CKX(cudaMemcpyAsync(info, x->d_info, sizeof(cuipm_info) * (size_t) nbatch, cudaMemcpyDeviceToHost, st));
-    CKX(cudaStreamSynchronize(st));
+    CK(cudaMemcpyAsync(sol_full, x->d_sol_full, sizeof(double) * x->lf->sol_stride * (size_t) nbatch, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(info, x->d_info, sizeof(cuipm_info) * (size_t) nbatch, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
     return CUIPM_OK;
 }
 

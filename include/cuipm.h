@@ -46,8 +46,8 @@ enum cuipm_error {
     CUIPM_ERR_INVALID = -1,     /* bad argument / unsupported option value */
     CUIPM_ERR_CUDA = -2,        /* CUDA runtime error (message via cuipm_last_error) */
     CUIPM_ERR_NO_DEVICE = -3,   /* no CUDA device: there is NO CPU fallback */
-    CUIPM_ERR_TOO_LARGE = -4    /* stage dimensions exceed what the kernel supports: the solver's vectors alone need more than
-                                 * 227 KB of shared memory, or a record needs offsets beyond 32 bits.  (Stage blocks that do not
+    CUIPM_ERR_TOO_LARGE = -4    /* stage dimensions exceed what the kernel supports: the solver's vectors alone need more shared
+                                 * memory than a block may have, or a record needs offsets beyond 32 bits.  (Stage blocks that do not
                                  * fit in shared memory are not refused: they go to a per-QP device scratch buffer.) */
 };
 

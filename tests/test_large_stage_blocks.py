@@ -1,6 +1,6 @@
 """Stage blocks that do not fit in shared memory: the generic kernel's global-scratch variant (run on an H100 with -m gpu).
 
-A shape whose stage-block buffers need more than the 227 KB of shared memory a block may have -- a condensed QP of the chain-mass,
+A shape whose stage-block buffers need more shared memory than a block may have -- a condensed QP of the chain-mass,
 quadrotor or legged shape under full condensing or a coarse cond_N -- runs the generic kernel with those buffers in a per-QP slice
 of a device scratch buffer, and the block condenser does the same with its scratch.  The tuning key "spill" = 1 forces the
 variant on a shape that fits; there it must reproduce the on-chip kernel bit for bit, since it performs the same arithmetic in
@@ -154,8 +154,10 @@ def _smem_kb(shape):
 @pytest.mark.parametrize("name,cond_N", [("c2", 1), ("c2", 2), ("c4", 1), ("c4", 3), ("c5", 1), ("c5", 5)])
 def test_refused_shapes_match_the_oracle(built, name, cond_N):
     from oracle import oracle_binding as ob
+    import torch
     _, _, cb = _condensed(name, cond_N, 8)
-    assert _smem_kb(cb.shape) > 227                 # the on-chip kernel cannot hold these blocks
+    # the on-chip kernel cannot hold these blocks: more than the device's whole opt-in limit, before its static shared memory
+    assert _smem_kb(cb.shape) * 1024 > torch.cuda.get_device_properties(0).shared_memory_per_block_optin
     o = default_opts()
     s = CuipmSolver(cb.shape, cb.nbatch)
     sol, info = s.solve(cb.qp, o)
@@ -170,7 +172,8 @@ def test_refused_shapes_match_the_oracle(built, name, cond_N):
 
 
 def test_vector_area_beyond_shared_memory_is_refused(built):
-    """What remains impossible: the vector area alone above 227 KB (here 4000 general constraints on one stage)."""
+    """What remains impossible: the vector area alone above the shared memory a block may have (here 4000 general constraints on
+    one stage)."""
     sh = P.random_shape(1, 2, 2, ng=4000)
     with pytest.raises(RuntimeError, match="vectors alone"):
         CuipmSolver(sh, 1)
