@@ -135,6 +135,16 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         f.restype = ip
     lib.cuipm_expand_device.argtypes = [vp, ip, vp, vp, vp, vp]
     lib.cuipm_expand_device.restype = ip
+    lib.cuipm_xcond_create.argtypes = [vp, ip, C.POINTER(C.c_int), ip, ip, ip]
+    lib.cuipm_xcond_create.restype = vp
+    lib.cuipm_xcond_destroy.argtypes = [vp]
+    lib.cuipm_xcond_solver.argtypes = [vp]
+    lib.cuipm_xcond_solver.restype = vp
+    for f in (lib.cuipm_xcond_solve_host, lib.cuipm_xcond_condense_rhs_and_solve_host):
+        f.argtypes = [vp, ip, vp, vp, vp, vp, C.POINTER(CuipmOpts)]
+        f.restype = ip
+    lib.cuipm_xcond_condense_lhs_host.argtypes = [vp, ip, vp]
+    lib.cuipm_xcond_condense_lhs_host.restype = ip
     lib.cuipm_set_tuning.argtypes = [vp, C.c_char_p, ip]
     lib.cuipm_set_tuning.restype = ip
     lib.cuipm_last_handed_back.argtypes = [vp]
@@ -339,43 +349,41 @@ class CuipmXcond:
 
     def __init__(self, full_shape: Shape, idxe0, cond_N: int, max_batch: int, device: int = 0):
         self.lib = load_library()
-        lib = self.lib
-        lib.cuipm_xcond_create.restype = C.c_void_p
-        lib.cuipm_xcond_create.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        lib.cuipm_xcond_destroy.argtypes = [C.c_void_p]
-        lib.cuipm_xcond_solve_host.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        lib.cuipm_xcond_condense_lhs_host.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
-        lib.cuipm_xcond_condense_rhs_and_solve_host.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         self.full_shape, self.layout = full_shape, Layout(full_shape)
         self._cshape = full_shape.as_ctypes()
         idx = (C.c_int * max(1, len(idxe0)))(*[int(i) for i in idxe0])
-        self.handle = lib.cuipm_xcond_create(C.byref(self._cshape), len(idxe0), idx, cond_N, max_batch, device)
+        self.handle = self.lib.cuipm_xcond_create(C.byref(self._cshape), len(idxe0), idx, cond_N, max_batch, device)
         if not self.handle:
-            raise RuntimeError("cuipm_xcond_create failed: " + lib.cuipm_last_error().decode())
+            raise RuntimeError("cuipm_xcond_create failed: " + self.lib.cuipm_last_error().decode())
 
-    def _run(self, fn, qp_full, opts, with_out=True):
-        qp_full = np.ascontiguousarray(qp_full, dtype=np.float64)
-        nb = qp_full.shape[0]
-        if not with_out:
-            rc = fn(self.handle, nb, qp_full.ctypes.data)
-            if rc != 0:
-                raise RuntimeError(self.lib.cuipm_last_error().decode())
-            return None
-        sol = np.zeros((nb, self.layout.sol_stride))
-        info = np.zeros(nb, dtype=INFO_DTYPE)
-        rc = fn(self.handle, nb, qp_full.ctypes.data, sol.ctypes.data, info.ctypes.data, C.byref(opts))
+    def _check(self, rc):
         if rc != 0:
             raise RuntimeError(self.lib.cuipm_last_error().decode())
-        return sol, info
 
-    def solve(self, qp_full, opts):
-        return self._run(self.lib.cuipm_xcond_solve_host, qp_full, opts)
+    def _solve(self, fn, qp_full, opts, want_stat):
+        qp_full = np.ascontiguousarray(qp_full, dtype=np.float64)
+        nb = qp_full.shape[0]
+        sol = np.zeros((nb, self.layout.sol_stride))
+        info = np.zeros(nb, dtype=INFO_DTYPE)
+        stat = np.zeros((nb, opts.stat_max + 1, STAT_M)) if want_stat else None
+        self._check(fn(self.handle, nb, qp_full.ctypes.data, sol.ctypes.data, info.ctypes.data,
+                       stat.ctypes.data if want_stat else None, C.byref(opts)))
+        return (sol, info, stat) if want_stat else (sol, info)
+
+    def solve(self, qp_full, opts: CuipmOpts, want_stat: bool = False):
+        """One pass: returns (sol, info[, stat]); with warm_start >= 2 the solve starts from this object's previous solution."""
+        return self._solve(self.lib.cuipm_xcond_solve_host, qp_full, opts, want_stat)
 
     def condense_lhs(self, qp_full):
-        return self._run(self.lib.cuipm_xcond_condense_lhs_host, qp_full, None, with_out=False)
+        qp_full = np.ascontiguousarray(qp_full, dtype=np.float64)
+        self._check(self.lib.cuipm_xcond_condense_lhs_host(self.handle, qp_full.shape[0], qp_full.ctypes.data))
 
-    def condense_rhs_and_solve(self, qp_full, opts):
-        return self._run(self.lib.cuipm_xcond_condense_rhs_and_solve_host, qp_full, opts)
+    def condense_rhs_and_solve(self, qp_full, opts: CuipmOpts, want_stat: bool = False):
+        return self._solve(self.lib.cuipm_xcond_condense_rhs_and_solve_host, qp_full, opts, want_stat)
+
+    @property
+    def last_kernel_ms(self) -> float:
+        return float(self.lib.cuipm_last_kernel_ms(self.lib.cuipm_xcond_solver(self.handle)))
 
     def close(self):
         if self.handle:
@@ -401,16 +409,7 @@ class CuipmReducer:
         self.handle = self.lib.cuipm_reducer_create(C.byref(self._cshape), len(idxe0), idx, device)
         if not self.handle:
             raise RuntimeError("cuipm_reducer_create failed: " + self.lib.cuipm_last_error().decode())
-        N = full_shape.N
-
-        class _CS(C.Structure):
-            _fields_ = [("N", C.c_int)] + [(n, C.POINTER(C.c_int)) for n in ("nx", "nu", "nb", "ng", "ns")] + \
-                       [("idxb", C.POINTER(C.POINTER(C.c_int))), ("idxs_rev", C.POINTER(C.POINTER(C.c_int)))]
-        cs = C.cast(self.lib.cuipm_reducer_reduced_shape(self.handle), C.POINTER(_CS)).contents
-        g = lambda a: [int(a[k]) for k in range(N + 1)]
-        nx, nu, nb, ng, ns = g(cs.nx), g(cs.nu), g(cs.nb), g(cs.ng), g(cs.ns)
-        self.reduced_shape = Shape(N, nx, nu, nb, ng, ns, [[int(cs.idxb[k][i]) for i in range(nb[k])] for k in range(N + 1)],
-                                   [[int(cs.idxs_rev[k][i]) for i in range(nb[k] + ng[k])] for k in range(N + 1)])
+        self.reduced_shape = _shape_from_c(self.lib.cuipm_reducer_reduced_shape(self.handle))
         self.full_layout, self.reduced_layout = Layout(full_shape), Layout(self.reduced_shape)
 
     def reduce(self, nbatch: int, d_qp_full: int, d_qp_red: int, stream: int = 0):

@@ -23,6 +23,8 @@ struct cuipm_xcond
     const cuipm_layout *lf = nullptr, *lr = nullptr;
     cuipm_layout *lc = nullptr;                        // layout of the condensed records (owned; null without condensing)
     double *d_full = nullptr, *d_red = nullptr, *d_cond = nullptr, *d_sol = nullptr, *d_sol_red = nullptr, *d_sol_full = nullptr;
+    double *d_stat = nullptr;                          // statistics tables, grown on demand
+    size_t stat_cap = 0;
     cuipm_info *d_info = nullptr;
     int lhs_valid = 0;
 };
@@ -38,7 +40,7 @@ extern "C" void cuipm_xcond_destroy(cuipm_xcond *x)
     if (x->red) cuipm_reducer_destroy(x->red);
     if (x->lc) cuipm_layout_destroy(x->lc);
     cudaFree(x->d_full); cudaFree(x->d_red); cudaFree(x->d_cond); cudaFree(x->d_sol); cudaFree(x->d_sol_red); cudaFree(x->d_sol_full);
-    cudaFree(x->d_info);
+    cudaFree(x->d_stat); cudaFree(x->d_info);
     delete x;
 }
 
@@ -72,7 +74,8 @@ extern "C" cuipm_xcond *cuipm_xcond_create(const cuipm_shape *full, int nbxe0, c
         || cudaMalloc(&x->d_sol, sizeof(double) * ls->sol_stride * nb) != cudaSuccess
         || (x->lc && cudaMalloc(&x->d_sol_red, sizeof(double) * x->lr->sol_stride * nb) != cudaSuccess)
         || cudaMalloc(&x->d_sol_full, sizeof(double) * x->lf->sol_stride * nb) != cudaSuccess
-        || cudaMalloc(&x->d_info, sizeof(cuipm_info) * nb) != cudaSuccess)
+        || cudaMalloc(&x->d_info, sizeof(cuipm_info) * nb) != cudaSuccess
+        || cudaMemset(x->d_sol, 0, sizeof(double) * ls->sol_stride * nb) != cudaSuccess)   // the first warm start starts from zeros
     {
         set_error("cuipm_xcond_create: device allocation failed (no CPU fallback)");
         return fail();
@@ -85,18 +88,28 @@ extern "C" int cuipm_xcond_cond_N(const cuipm_xcond *x) { return x ? x->cond_N :
 extern "C" cuipm_solver *cuipm_xcond_solver(cuipm_xcond *x) { return x ? x->solver : nullptr; }
 
 // mode 0: one pass; 1: preparation phase only (reduce + condense_lhs); 2: feedback phase (reduce + condense_rhs + solve + ...)
-static int chain(cuipm_xcond *x, int mode, int nbatch, const double *qp_full, double *sol_full, cuipm_info *info, const cuipm_opts *opts)
+// d_sol holds the solver's (reduced or condensed) solution of the previous call: warm starts (warm_start >= 2) start from it
+static int chain(cuipm_xcond *x, int mode, int nbatch, const double *qp_full, double *sol_full, cuipm_info *info, double *stat,
+                 const cuipm_opts *opts)
 {
     if (!x || nbatch < 0 || nbatch > x->max_batch || !qp_full || (mode != 1 && (!sol_full || !info || !opts)))
     {
         set_error("cuipm_xcond: bad arguments (nbatch must be <= max_batch)");
         return CUIPM_ERR_INVALID;
     }
-    if (mode != 1 && opts->warm_start >= 2) { set_error("cuipm_xcond: warm starts (warm_start >= 2) are not carried through the chain"); return CUIPM_ERR_INVALID; }
     if (mode == 2 && x->cond && x->lhs_valid < nbatch) { set_error("cuipm_xcond_condense_rhs_and_solve_host: call cuipm_xcond_condense_lhs_host first"); return CUIPM_ERR_INVALID; }
     if (nbatch == 0) return CUIPM_OK;
     CK(cudaSetDevice(x->device));
     cudaStream_t st = (cudaStream_t) cuipm_stream(x->solver);
+    const size_t stat_n = stat ? (size_t) nbatch * CUIPM_STAT_M * (opts->stat_max + 1) : 0;
+    if (x->stat_cap < stat_n)
+    {
+        CK(cudaStreamSynchronize(st));
+        cudaFree(x->d_stat);
+        x->d_stat = nullptr;
+        CK(cudaMalloc(&x->d_stat, sizeof(double) * stat_n));
+        x->stat_cap = stat_n;
+    }
     CK(cudaMemcpyAsync(x->d_full, qp_full, sizeof(double) * x->lf->qp_stride * (size_t) nbatch, cudaMemcpyHostToDevice, st));
     RCX(cuipm_reduce_device(x->red, nbatch, x->d_full, x->d_red, st));
     const double *d_qp = x->d_red;
@@ -108,7 +121,7 @@ static int chain(cuipm_xcond *x, int mode, int nbatch, const double *qp_full, do
         d_qp = x->d_cond;
     }
     if (mode == 1) { CK(cudaStreamSynchronize(st)); return CUIPM_OK; }
-    RCX(cuipm_solve_device(x->solver, nbatch, d_qp, x->d_sol, x->d_info, nullptr, opts, 0));
+    RCX(cuipm_solve_device(x->solver, nbatch, d_qp, x->d_sol, x->d_info, stat ? x->d_stat : nullptr, opts, 0));
     const double *d_sr = x->d_sol;
     if (x->cond)
     {
@@ -118,20 +131,22 @@ static int chain(cuipm_xcond *x, int mode, int nbatch, const double *qp_full, do
     RCX(cuipm_restore_device(x->red, nbatch, x->d_full, d_sr, x->d_sol_full, opts->lam_min, opts->t_min, st));
     CK(cudaMemcpyAsync(sol_full, x->d_sol_full, sizeof(double) * x->lf->sol_stride * (size_t) nbatch, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(info, x->d_info, sizeof(cuipm_info) * (size_t) nbatch, cudaMemcpyDeviceToHost, st));
+    if (stat) CK(cudaMemcpyAsync(stat, x->d_stat, sizeof(double) * stat_n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     return CUIPM_OK;
 }
 
-extern "C" int cuipm_xcond_solve_host(cuipm_xcond *x, int nbatch, const double *qp_full, double *sol_full, cuipm_info *info, const cuipm_opts *opts)
+extern "C" int cuipm_xcond_solve_host(cuipm_xcond *x, int nbatch, const double *qp_full, double *sol_full, cuipm_info *info, double *stat,
+                                      const cuipm_opts *opts)
 {
-    return chain(x, 0, nbatch, qp_full, sol_full, info, opts);
+    return chain(x, 0, nbatch, qp_full, sol_full, info, stat, opts);
 }
 extern "C" int cuipm_xcond_condense_lhs_host(cuipm_xcond *x, int nbatch, const double *qp_full)
 {
-    return chain(x, 1, nbatch, qp_full, nullptr, nullptr, nullptr);
+    return chain(x, 1, nbatch, qp_full, nullptr, nullptr, nullptr, nullptr);
 }
 extern "C" int cuipm_xcond_condense_rhs_and_solve_host(cuipm_xcond *x, int nbatch, const double *qp_full, double *sol_full, cuipm_info *info,
-                                                       const cuipm_opts *opts)
+                                                       double *stat, const cuipm_opts *opts)
 {
-    return chain(x, 2, nbatch, qp_full, sol_full, info, opts);
+    return chain(x, 2, nbatch, qp_full, sol_full, info, stat, opts);
 }

@@ -8,16 +8,18 @@
 identical QPs, one launch.
 
 What happens between the user's QP and the kernel is what the reference's xcond layer does for
-PARTIAL_CONDENSING_HPIPM with N2 = N (acados/ocp_qp/ocp_qp_partial_condensing.c:523-689): the stage-0 state
-bounds marked as equalities (``idxe``: x0 = lbx_0) are eliminated before the solve (d_ocp_qp_reduce_eq_dof,
-external/hpipm/ocp_qp/x_ocp_qp_red.c:278-560) and restored afterwards, multipliers included
-(d_ocp_qp_restore_eq_dof, :848-994) -- here vectorised over the batch in numpy -- and the data are packed into the
-cuipm QP records (include/cuipm.h, HPIPM's conventions: BAt = [B'; A'], RSQ = [R S; S' Q] lower,
-DCt = [D'; C'], d = [lb, lg, -ub, -ug, lls, lus]).  Block condensing with cond_N < N is acados_b200/condensing.py
-(the same module restated on the host, records to records); on the GPU the uncondensed QP is usually the cheaper one
-to factorise, so cond_N defaults to N as in the reference.
+PARTIAL_CONDENSING_HPIPM (acados/ocp_qp/ocp_qp_xcond_solver.c:523-669 in front of ocp_qp_partial_condensing.c:523-689):
+the stage-0 state bounds marked as equalities (``idxe``: x0 = lbx_0) are eliminated before the solve
+(d_ocp_qp_reduce_eq_dof, external/hpipm/ocp_qp/x_ocp_qp_red.c:278-560), the QP is block-condensed to cond_N stages if
+cond_N < N, and after the solve the solution is expanded and the eliminated states are restored, multipliers included
+(d_ocp_qp_restore_eq_dof, :848-994).  The data are packed into the cuipm QP records (include/cuipm.h, HPIPM's
+conventions: BAt = [B'; A'], RSQ = [R S; S' Q] lower, DCt = [D'; C'], d = [lb, lg, -ub, -ug, lls, lus]); on the GPU
+the uncondensed QP is usually the cheaper one to factorise, so cond_N defaults to N as in the reference.
 
-The solve itself is the CUDA path behind the C ABI (binding.CuipmSolver): no CPU fallback.
+By default the records travel as posed and that whole chain runs on the device in one cuipm_xcond object
+(binding.CuipmXcond, acados_b200/csrc/cuipm_xcond.cu).  ``device_reduce=False`` runs the elimination and the restore
+here, vectorised over the batch in numpy, and the condensing in acados_b200/condensing.py, and solves the records with
+binding.CuipmSolver; the tests hold the device route to it.  Either way the solve is CUDA: no CPU fallback.
 """
 from __future__ import annotations
 
@@ -27,7 +29,7 @@ from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
-from .binding import STAT_M, CuipmOpts, CuipmSolver, default_opts
+from .binding import STAT_M, CuipmOpts, CuipmSolver, CuipmXcond, default_opts
 from .problems import Layout, Shape
 
 DYNAMICS_FIELDS = ("A", "B", "b")
@@ -397,47 +399,36 @@ class OcpQpBatchSolver:
     """Solves a batch of structurally identical QPs in one launch of the CUDA path."""
 
     def __init__(self, qps: Sequence[OcpQp], opts: Optional[OcpQpOptions] = None, device: int = 0, device_reduce: bool = True):
-        """device_reduce: run the stage-0 equality elimination and the restore on the GPU (cuipm_reduce_device /
-        cuipm_restore_device): the records travel as posed, the reduced records never exist on the host.  False keeps
-        both on the host (numpy)."""
+        """device_reduce: run the whole chain -- stage-0 equality elimination, block condensing for cond_N < N, solve, expansion
+        and restore -- on the GPU in one cuipm_xcond object (binding.CuipmXcond): the records travel as posed, the reduced and
+        condensed records never exist on the host.  False runs the elimination, the restore and the condensing on the host
+        (numpy) and solves with binding.CuipmSolver."""
         self.opts = opts or OcpQpOptions()
         self.opts.make_consistent(qps[0].N)
         self.device, self.device_reduce = device, device_reduce
         self.c_opts = self.opts.to_cuipm()
-        self._reducer = None
-        self._dcond = None
+        self._cond_N = self.opts.cond_N if self.opts.cond_N is not None else qps[0].N
         self._load(qps)
-        if self._dcond is not None:
-            solve_shape = self._dcond.condensed_shape
-        elif self._cond is not None:
-            solve_shape = self._cond.cshape
+        if device_reduce:
+            self._solver = CuipmXcond(self.packed.shape, self._idxe0, self._cond_N, len(qps), device)
         else:
-            solve_shape = self._reducer.reduced_shape if self.device_reduce else self.packed.shape
-        self._solver = CuipmSolver(solve_shape, len(qps), device)
+            self._solver = CuipmSolver(self._cond.cshape if self._cond is not None else self.packed.shape, len(qps), device)
         self._sol = None
         self.info = None
         self.stat = None
         self.result = None
 
     def _load(self, qps):
-        N = qps[0].N
         self._idxe0 = [int(i) for i in qps[0].idxe[0]]
-        cond_N = self.opts.cond_N if self.opts.cond_N is not None else N
         self._cond = None
         if self.device_reduce:
-            # records travel as posed; elimination, block condensing, expansion and restore all run on the GPU
-            from .binding import CuipmCondenser, CuipmReducer
-            self.packed = PackedBatch(qps, eliminate=False)
-            if self._reducer is None:
-                self._reducer = CuipmReducer(self.packed.shape, [int(i) for i in qps[0].idxe[0]], self.device)
-            if cond_N < N and self._dcond is None:
-                self._dcond = CuipmCondenser(self._reducer.reduced_shape, cond_N, self.device)
+            self.packed = PackedBatch(qps, eliminate=False)          # records as posed
         else:
             self.packed = PackedBatch(qps)
-            if cond_N < N:
-                # the same on the host (acados_b200/condensing.py, numpy)
+            if self._cond_N < self.packed.N:
+                # block condensing on the host (acados_b200/condensing.py, numpy)
                 from .condensing import BlockCondenser
-                self._cond = BlockCondenser(self.packed.shape, cond_N)
+                self._cond = BlockCondenser(self.packed.shape, self._cond_N)
                 self._cqp = self._cond.condense(self.packed.qp)
 
     @property
@@ -445,9 +436,9 @@ class OcpQpBatchSolver:
         return self.packed.N
 
     def update(self, qps: Sequence[OcpQp]):
-        """New data, same structure (an SQP / RL sweep re-solving with updated linearisations).  The reducer, the condenser
-        and the solver hold index maps and buffers of the structure they were built for: a batch of another size, other
-        dimensions, bound / slack index maps or stage-0 equalities is refused rather than solved with stale maps."""
+        """New data, same structure (an SQP / RL sweep re-solving with updated linearisations).  The device chain and the solver
+        hold index maps and buffers of the structure they were built for: a batch of another size, other dimensions, bound /
+        slack index maps or stage-0 equalities is refused rather than solved with stale maps."""
         old, old_idxe, old_nb = self.packed.shape, [int(i) for i in self._idxe0], self.packed.nbatch
         self._load(qps)
         new = self.packed.shape
@@ -459,70 +450,41 @@ class OcpQpBatchSolver:
             raise ValueError("OcpQpBatchSolver.update: the new batch does not have the structure (batch size, dimensions, idxb, "
                              "idxs_rev, idxe) this solver was built for; create a new solver")
 
+    def _require_device_condensing(self, name):
+        if not (self.device_reduce and self._cond_N < self.N):
+            raise RuntimeError(f"{name}: needs the device path with cond_N < N")
+
     def condense_lhs(self) -> None:
         """Preparation phase of an SQP-RTI step (``ocp_qp_xcond_solver``'s condense_lhs, ocp_qp_xcond_solver.c:591-627): the QPs
         loaded last are reduced and condensed on the device and the condensed records -- with the prediction matrices of every
         stage -- stay there.  Device path with cond_N < N only."""
-        if not (self.device_reduce and self._dcond is not None):
-            raise RuntimeError("condense_lhs: needs the device path with cond_N < N")
-        self.solve(_lhs_only=True)
+        self._require_device_condensing("condense_lhs")
+        self._solver.condense_lhs(self.packed.qp)
 
     def condense_rhs_and_solve(self) -> np.ndarray:
         """Feedback phase (``condense_rhs_and_solve``, ocp_qp_xcond_solver.c:629-669): the QPs loaded last (``update``: same
         matrices as at ``condense_lhs``, new vectors) refresh the vectors of the resident condensed records, which are then solved
         and expanded.  Returns the acados status per QP."""
-        if not (self.device_reduce and self._dcond is not None and getattr(self, "_d_cond", None) is not None):
-            raise RuntimeError("condense_rhs_and_solve: call condense_lhs first (device path, cond_N < N)")
-        return self.solve(_rhs_only=True)
+        self._require_device_condensing("condense_rhs_and_solve")
+        sol, self.info, self.stat = self._solver.condense_rhs_and_solve(self.packed.qp, self.c_opts, want_stat=True)
+        self.result = self.packed.unpack(sol)
+        return self._status()
 
-    def solve(self, _lhs_only: bool = False, _rhs_only: bool = False) -> np.ndarray:
-        """Returns the acados status per QP (0 success, 2 max iter, 3 min step, 1 NaN; ocp_qp_hpipm.c:398-404)."""
-        lhs_only, rhs_only = _lhs_only, _rhs_only
-        warm = self._sol if (self.c_opts.warm_start >= 2 and self._sol is not None) else None
-        if self._cond is not None:
-            self._sol, self.info, self.stat = self._solver.solve(self._cqp, self.c_opts, sol0=warm, want_stat=True)
-            self.result = self.packed.unpack(self._cond.expand(self.packed.qp, self._sol), self.c_opts.lam_min, self.c_opts.t_min)
-        elif not self.device_reduce:
-            self._sol, self.info, self.stat = self._solver.solve(self.packed.qp, self.c_opts, sol0=warm, want_stat=True)
-            self.result = self.packed.unpack(self._sol, self.c_opts.lam_min, self.c_opts.t_min)
-        else:
-            import torch   # device buffers and copies only
-            from .binding import INFO_DTYPE
-            nb, red, dc, o = self.packed.nbatch, self._reducer, self._dcond, self.c_opts
-            dev = torch.device("cuda", self.device)
-            st = self._solver.lib.cuipm_stream(self._solver.handle)
-            slay = dc.condensed_layout if dc is not None else red.reduced_layout          # layout the solver works on
-            d_full = torch.from_numpy(self.packed.qp).to(dev)
-            d_red = torch.empty((nb, red.reduced_layout.qp_stride), dtype=torch.float64, device=dev)
-            d_qp = d_red if dc is None else torch.empty((nb, slay.qp_stride), dtype=torch.float64, device=dev)
-            d_sol = torch.zeros((nb, slay.sol_stride), dtype=torch.float64, device=dev) if warm is None else torch.from_numpy(warm).to(dev)
-            d_info = torch.zeros(nb * INFO_DTYPE.itemsize, dtype=torch.uint8, device=dev)
-            d_stat = torch.zeros((nb, o.stat_max + 1, STAT_M), dtype=torch.float64, device=dev)
-            d_sol_red = d_sol if dc is None else torch.empty((nb, red.reduced_layout.sol_stride), dtype=torch.float64, device=dev)
-            d_sol_full = torch.empty((nb, red.full_layout.sol_stride), dtype=torch.float64, device=dev)
-            torch.cuda.synchronize(dev)
-            red.reduce(nb, d_full.data_ptr(), d_red.data_ptr(), st)
-            if dc is not None:
-                if rhs_only:
-                    # feedback phase: the condensed records of the preparation phase stay on the device, only their vectors
-                    # are refreshed (cuipm_condense_rhs_device, O(nx^2 + nx n2) per stage)
-                    d_qp = self._d_cond
-                    dc.condense_rhs(nb, d_red.data_ptr(), d_qp.data_ptr(), st)
-                else:
-                    dc.condense_lhs(nb, d_red.data_ptr(), d_qp.data_ptr(), st)
-                    self._d_cond = d_qp
-            if lhs_only:
-                torch.cuda.synchronize(dev)
-                return None
-            self._solver.solve_device(nb, d_qp.data_ptr(), d_sol.data_ptr(), d_info.data_ptr(), o, sync=False, d_stat=d_stat.data_ptr())
-            if dc is not None:
-                dc.expand(nb, d_red.data_ptr(), d_sol.data_ptr(), d_sol_red.data_ptr(), st)
-            red.restore(nb, d_full.data_ptr(), d_sol_red.data_ptr(), d_sol_full.data_ptr(), o.lam_min, o.t_min, st)
-            self._solver.wait()
-            self._sol = d_sol.cpu().numpy()
-            self.info = np.frombuffer(d_info.cpu().numpy().tobytes(), dtype=INFO_DTYPE).copy()
-            self.stat = d_stat.cpu().numpy()
-            self.result = self.packed.unpack(d_sol_full.cpu().numpy())
+    def solve(self) -> np.ndarray:
+        """Returns the acados status per QP (0 success, 2 max iter, 3 min step, 1 NaN; ocp_qp_hpipm.c:398-404).  With
+        warm_start >= 2 the solve starts from the previous solve's solution in the solver's (reduced or condensed) layout."""
+        if self.device_reduce:
+            sol, self.info, self.stat = self._solver.solve(self.packed.qp, self.c_opts, want_stat=True)
+            self.result = self.packed.unpack(sol)
+            return self._status()
+        warm = self._sol if self.c_opts.warm_start >= 2 else None
+        qp = self._cqp if self._cond is not None else self.packed.qp
+        self._sol, self.info, self.stat = self._solver.solve(qp, self.c_opts, sol0=warm, want_stat=True)
+        sol = self._cond.expand(self.packed.qp, self._sol) if self._cond is not None else self._sol
+        self.result = self.packed.unpack(sol, self.c_opts.lam_min, self.c_opts.t_min)
+        return self._status()
+
+    def _status(self) -> np.ndarray:
         return np.array([{0: 0, 1: 2, 2: 3, 3: 1, 4: 9}.get(int(s), -1) for s in self.info["status"]])
 
     def get(self, stage: int, field: str) -> np.ndarray:
@@ -543,10 +505,6 @@ class OcpQpBatchSolver:
 
     def close(self):
         self._solver.close()
-        if self._reducer is not None:
-            self._reducer.close()
-        if self._dcond is not None:
-            self._dcond.close()
 
 
 class OcpQpSolver:

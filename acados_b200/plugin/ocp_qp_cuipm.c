@@ -527,8 +527,8 @@ int ocp_qp_cuipm_xcond_batch_solve(ocp_qp_cuipm_xcond_batch *c, int n, ocp_qp_in
     for (int i = 0; i < n; i++) pack_qp(qp_in[i], l, c->b_qp + l->qp_stride * (size_t) i);
     int rc;
     if (phase == 1) rc = cuipm_xcond_condense_lhs_host(c->x, n, c->b_qp);
-    else if (phase == 2) rc = cuipm_xcond_condense_rhs_and_solve_host(c->x, n, c->b_qp, c->b_sol, c->b_info, &opts->c);
-    else rc = cuipm_xcond_solve_host(c->x, n, c->b_qp, c->b_sol, c->b_info, &opts->c);
+    else if (phase == 2) rc = cuipm_xcond_condense_rhs_and_solve_host(c->x, n, c->b_qp, c->b_sol, c->b_info, NULL, &opts->c);
+    else rc = cuipm_xcond_solve_host(c->x, n, c->b_qp, c->b_sol, c->b_info, NULL, &opts->c);
     if (rc != CUIPM_OK) { printf("\nerror: ocp_qp_cuipm_xcond_batch_solve: %s\n", cuipm_last_error()); exit(1); }
     if (phase == 1) return ACADOS_SUCCESS;
     const double t_solve = acados_toc(&timer);

@@ -79,6 +79,8 @@ int ocp_qp_cuipm_batch_solve(void *config, int n, ocp_qp_in **qp_in, ocp_qp_out 
  * (cuipm_xcond_*, include/cuipm.h) -- the batched counterpart of ocp_qp_xcond_solver's evaluate (ocp_qp_xcond_solver.c:523-589)
  * with acados' CPU condensing module taken out of the path.  phase: 0 = one pass; 1 = condense_lhs only (:591-627, nothing is
  * written to qp_out); 2 = condense_rhs_and_solve (:629-669) on QPs whose matrices are those of the last phase-1 call.
+ * With warm_start >= 2 a solve starts from the context's previous condensed solution (zeros before the first), as
+ * ocp_qp_xcond_solver does with its xcond_qp_out (:554-569); the qp_out structs are not read.
  * The context owns the device objects and the page-locked staging. */
 typedef struct ocp_qp_cuipm_xcond_batch ocp_qp_cuipm_xcond_batch;
 ocp_qp_cuipm_xcond_batch *ocp_qp_cuipm_xcond_batch_create(ocp_qp_in *qp_in0, int n_max, int cond_N, int device);

@@ -268,18 +268,22 @@ int cuipm_condense_rhs_device(cuipm_condenser *c, int nbatch, const double *d_qp
  * evaluate() in one piece or split into condense_lhs (:591-627, preparation phase of SQP-RTI) and condense_rhs_and_solve
  * (:629-669, feedback phase).  `full` is the shape as the user poses it, idxe0 as for cuipm_reducer_create; cond_N in 1..N
  * (<= 0 or N: no block condensing).  Records of the full shape come from (page-locked) host memory, solutions of the full
- * shape and the per-QP summaries go back; the reduced / condensed records, the prediction matrices of the lhs pass and all
- * intermediate solutions live on the device.  warm_start >= 2 is refused (the chain does not map a full-shape iterate forward). */
+ * shape, the per-QP summaries and, if `stat` is not NULL, the statistics tables (as for cuipm_solve_host) go back; the reduced /
+ * condensed records, the prediction matrices of the lhs pass and all intermediate solutions live on the device.  With
+ * warm_start >= 2 the solve starts from this object's previous solution in the reduced / condensed layout (zeros before the
+ * first solve), as the reference runs its QP solver on the condensed solution of the previous call unless
+ * initialize_next_xcond_qp_from_qp_out is set (ocp_qp_xcond_solver.c:554-569). */
 typedef struct cuipm_xcond cuipm_xcond;
 cuipm_xcond *cuipm_xcond_create(const cuipm_shape *full, int nbxe0, const int *idxe0, int cond_N, int max_batch, int device);
 void cuipm_xcond_destroy(cuipm_xcond *x);
 const cuipm_layout *cuipm_xcond_full_layout(const cuipm_xcond *x);
 int cuipm_xcond_cond_N(const cuipm_xcond *x);
 cuipm_solver *cuipm_xcond_solver(cuipm_xcond *x);      /* the solver of the reduced / condensed shape (statistics, getters); owned by x */
-int cuipm_xcond_solve_host(cuipm_xcond *x, int nbatch, const double *qp_full, double *sol_full, cuipm_info *info, const cuipm_opts *opts);
+int cuipm_xcond_solve_host(cuipm_xcond *x, int nbatch, const double *qp_full, double *sol_full, cuipm_info *info, double *stat,
+                           const cuipm_opts *opts);
 int cuipm_xcond_condense_lhs_host(cuipm_xcond *x, int nbatch, const double *qp_full);
 int cuipm_xcond_condense_rhs_and_solve_host(cuipm_xcond *x, int nbatch, const double *qp_full, double *sol_full, cuipm_info *info,
-                                            const cuipm_opts *opts);
+                                            double *stat, const cuipm_opts *opts);
 
 /* Riccati quantities of the last factorisation (reference: ocp_qp_hpipm_solver_get, ocp_qp_hpipm.c:417-478).
  * field in {"P","p","K","k","Lr"}; copies column-major data of QP `iqp`, stage `stage` into `value`. */

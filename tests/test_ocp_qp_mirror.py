@@ -248,6 +248,51 @@ def test_batch_solver_gpu(built):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("warm_start,cond_N", [(2, None), (3, None), (2, 3), (3, 3)])
+def test_warm_start_through_the_front_end_gpu(built, warm_start, cond_N):
+    """warm_start >= 2: a solve starts from the previous solve's solution in the solver's (reduced or condensed) layout, as the
+    reference's xcond solver does (ocp_qp_xcond_solver.c:554-569).  Solve, update with new vectors, solve again: the device route
+    (cuipm_xcond) and the host route agree on iteration counts and solutions, and the second solve is not a cold one."""
+    import copy
+    from acados_b200.ocp_qp import OcpQpBatchSolver
+    # the routes' first solutions differ in the last bits (see test_batch_solver_gpu); warm_start = 3 restarts from multipliers
+    # clamped at lam0_min, which at the default tolerances leaves the routes ~1e-8 apart, so both run to 1e-10; a QP right at
+    # the stopping threshold could still take one iteration more on one route: these instances have none
+    tight = dict(tol_stat=1e-10, tol_eq=1e-10, tol_ineq=1e-10, tol_comp=1e-10)
+    rng = np.random.default_rng(6)
+    qps = [random_ocp_qp(rng) for _ in range(16)]
+    new = copy.deepcopy(qps)
+    for qp in new:
+        x0 = qp.lbx[0] + 0.05 * rng.standard_normal(qp.lbx[0].shape)
+        qp.set("lbx", 0, x0); qp.set("ubx", 0, x0)
+        for k in range(qp.N + 1):
+            qp.set("q", k, qp.q[k] + 0.05 * rng.standard_normal(qp.q[k].shape))
+            if k < qp.N:
+                qp.set("b", k, qp.b[k] + 0.01 * rng.standard_normal(qp.b[k].shape))
+    routes = [OcpQpBatchSolver(qps, OcpQpOptions(warm_start=warm_start, cond_N=cond_N, **tight), device_reduce=d) for d in (True, False)]
+    for bs in routes:
+        # the first solve runs cold: from zeros, warm_start = 3 clamps the multipliers to lam0_min and stops at the minimal step
+        bs.c_opts.warm_start = 0
+        assert (bs.solve() == 0).all()
+        bs.c_opts.warm_start = warm_start
+        bs.update(new)
+        bs.solve()
+    bs, bh = routes
+    assert np.array_equal(bs.info["status"], bh.info["status"]) and (bs.info["status"] == 0).sum() >= 12
+    assert np.array_equal(bs.get_stats("iter"), bh.get_stats("iter"))
+    ok = bs.info["status"] == 0
+    for k in range(bs.N + 1):
+        for f in ("u", "x", "sl", "su"):
+            assert np.allclose(bs.get(k, f)[ok], bh.get(k, f)[ok], rtol=0, atol=1e-9), (k, f)
+        for f in ("lam", "t"):
+            assert np.allclose(bs.get(k, f)[ok], bh.get(k, f)[ok], rtol=1e-6, atol=1e-8), (k, f)
+    cold = OcpQpBatchSolver(new, OcpQpOptions(cond_N=cond_N, **tight))
+    cold.solve()
+    assert any(not np.array_equal(bs.get(k, "u"), cold.get(k, "u")) for k in range(bs.N))
+    bs.close(); bh.close(); cold.close()
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("soft,general", [(False, False), (True, True)])
 def test_device_elimination_matches_host(built, soft, general):
     """cuipm_reduce_device / cuipm_restore_device (the batched reduce_eq_dof / restore_eq_dof of row a15) against the

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 from acados_b200 import problems as P
-from acados_b200.binding import CuipmSolver, CuipmXcond, default_opts
+from acados_b200.binding import CuipmSolver, default_opts
 from acados_b200.ocp_qp import OcpQpBatchSolver, OcpQpOptions, PackedBatch
 from test_large_stage_blocks import _smem_kb
 from test_ocp_qp_mirror import random_ocp_qp
@@ -54,18 +54,19 @@ def _legged_qps(n=4, seed=11):
 
 
 def _front_end_result(bs):
-    return [np.copy(bs.get(k, f)) for k in range(bs.N + 1) for f in ("u", "x", "lam")] + [bs.info.copy()]
+    return [np.copy(bs.get(k, f)) for k in range(bs.N + 1) for f in ("u", "x", "lam")] + [bs.info.copy(), bs.stat.copy()]
 
 
 def test_condensed_front_end_solvers_of_two_shapes(built):
     """The legged shape at cond_N = 5 keeps 94 KB of condenser scratch on chip (above the 48 KB a launch gets without the
-    attribute); at cond_N = 1 it needs 277 KB, in global memory.  Creating and using the second solver leaves the first one's
-    solve bit-identical."""
+    attribute); at cond_N = 1 it needs 277 KB, in global memory.  Creating and using the second solver (a second cuipm_xcond
+    chain) leaves the first one's solve bit-identical."""
     import torch
     qps = _legged_qps()
     optin = torch.cuda.get_device_properties(0).shared_memory_per_block_optin
+    reduced = PackedBatch(qps).shape
     a = OcpQpBatchSolver(qps, OcpQpOptions(cond_N=5))
-    scratch_a = _condenser_scratch_bytes(a._reducer.reduced_shape, 5)
+    scratch_a = _condenser_scratch_bytes(reduced, 5)
     # above the 48 KB a launch may have without the attribute, and on chip: the condenser compares its scratch with the opt-in
     # limit less its kernels' static shared memory, which is 0 B for condense_kernel and expand_kernel (-Xptxas -v); the 16 KB
     # margin only keeps the assertion independent of that figure
@@ -73,23 +74,8 @@ def test_condensed_front_end_solvers_of_two_shapes(built):
     a.solve()
     ref = _front_end_result(a)
     b = OcpQpBatchSolver(qps, OcpQpOptions(qp_solver="FULL_CONDENSING_HPIPM"))
-    assert _condenser_scratch_bytes(b._reducer.reduced_shape, 1) > optin
+    assert _condenser_scratch_bytes(reduced, 1) > optin
     b.solve()
     a.solve()
     assert all(np.ascontiguousarray(x).tobytes() == np.ascontiguousarray(y).tobytes() for x, y in zip(ref, _front_end_result(a)))
     a.close(); b.close()
-
-
-def test_xcond_chains_of_two_shapes(built):
-    """The same through cuipm_xcond_*: a second chain with its condenser scratch in global memory leaves the first bit-identical."""
-    qps = _legged_qps()
-    full = PackedBatch(qps, eliminate=False)
-    idxe0 = [int(i) for i in qps[0].idxe[0]]
-    o = default_opts()
-    xa = CuipmXcond(full.shape, idxe0, 5, len(qps))
-    sol0, info0 = xa.solve(full.qp, o)
-    xb = CuipmXcond(full.shape, idxe0, 1, len(qps))
-    xb.solve(full.qp, o)
-    sol1, info1 = xa.solve(full.qp, o)
-    assert sol0.tobytes() == sol1.tobytes() and info0.tobytes() == info1.tobytes()
-    xa.close(); xb.close()
