@@ -40,7 +40,6 @@ struct cuipm_solver
     int last_launches = 0;
     int pending = 0;                         // an asynchronous host solve has been enqueued and not waited for
     float last_ms = 0.f;
-    cuipm_opts last_opts{};
     GenericPath generic;                     // generic kernel (cuipm_kernel.cu)
     FastPath fast;                           // throughput kernel (cuipm_fast.cu)
     cudaEvent_t evk0 = nullptr, evk1 = nullptr;   // around the throughput kernel of the last cuipm_solve_device call
@@ -72,6 +71,22 @@ int cuda_error(const std::string &what, int err)
     return CUIPM_ERR_CUDA;
 }
 
+double *stat_buffer(cuipm_solver *s, size_t n)
+{
+    if (s->stat_cap >= n) return s->d_stat;
+    cudaError_t e = cudaStreamSynchronize(s->stream);
+    if (e == cudaSuccess)
+    {
+        cudaFree(s->d_stat);
+        s->d_stat = nullptr;
+        s->stat_cap = 0;
+        e = cudaMalloc(&s->d_stat, sizeof(double) * n);
+    }
+    if (e != cudaSuccess) { cuda_error("statistics buffer", (int) e); return nullptr; }
+    s->stat_cap = n;
+    return s->d_stat;
+}
+
 }  // namespace cuipm
 
 static int build_desc(cuipm_solver *s, const cuipm_shape *sh)
@@ -93,11 +108,8 @@ static int build_desc(cuipm_solver *s, const cuipm_shape *sh)
 // One batch (or one chunk of it) on `stream`: the throughput kernel where the shape and the options allow it, then the
 // generic kernel over the QPs it handed back (cold paths); otherwise the generic kernel over everything.
 // slot selects the hand-back counter (chunks run concurrently on different streams).
-static int launch_batch(cuipm_solver *s, const LaunchArgs &a0, int slot, size_t lo, cudaStream_t stream, int *launches)
+static int launch_batch(cuipm_solver *s, LaunchArgs a, int slot, size_t lo, cudaStream_t stream, int *launches)
 {
-    LaunchArgs a = a0;
-    a.redo_list = nullptr;
-    a.redo_count = nullptr;
     const bool timed = slot == 0 && s->evk0;
     int rc = s->fast.enqueue(a, lo, slot, (void *) stream, launches, timed ? s->evk0 : nullptr, timed ? s->evk1 : nullptr);
     if (rc != CUIPM_OK) return rc;
@@ -105,6 +117,37 @@ static int launch_batch(cuipm_solver *s, const LaunchArgs &a0, int slot, size_t 
     rc = s->generic.solve(a, lo, (void *) stream);
     if (rc != CUIPM_OK) return rc;
     (*launches)++;
+    return CUIPM_OK;
+}
+
+// Launch arguments for records lo .. lo+n-1 of qp / sol / info / stat (given from record lo on) and of the solver's work records
+static LaunchArgs launch_args(const cuipm_solver *s, size_t lo, int n, const double *qp, double *sol, cuipm_info *info, double *stat,
+                              const cuipm_opts *opts)
+{
+    LaunchArgs a{};
+    a.P = s->P; a.sd = s->d_sd; a.ipool = s->d_ipool; a.qp = qp; a.sol = sol; a.work = s->d_work + s->P.work_stride * lo;
+    a.info = info; a.stat = stat; a.o = *opts; a.nbatch = n;
+    return a;
+}
+
+// Records lo .. lo+n-1 of the host buffers (stat: if not null, through the solver's statistics buffer) copied in, solved and copied
+// out on pipe stream `slot`, then pipe_done[slot].  Threads enqueue slots concurrently: no solver-wide writes beyond launch_batch's.
+static int enqueue_chunk(cuipm_solver *s, int slot, int lo, int n, const double *qp, double *sol, cuipm_info *info, double *stat,
+                         const cuipm_opts *opts, int *launches)
+{
+    cudaStream_t st = s->pipe[slot];
+    const size_t qo = s->P.qp_stride * (size_t) lo, so = s->P.sol_stride * (size_t) lo;
+    const size_t srow = (size_t) CUIPM_STAT_M * (opts->stat_max + 1), to = srow * lo;
+    CK(cudaMemcpyAsync(s->d_qp + qo, qp + qo, sizeof(double) * s->P.qp_stride * n, cudaMemcpyHostToDevice, st));
+    if (opts->warm_start >= 1)
+        CK(cudaMemcpyAsync(s->d_sol + so, sol + so, sizeof(double) * s->P.sol_stride * n, cudaMemcpyHostToDevice, st));
+    const LaunchArgs a = launch_args(s, lo, n, s->d_qp + qo, s->d_sol + so, s->d_info + lo, stat ? s->d_stat + to : nullptr, opts);
+    int rc = launch_batch(s, a, slot, (size_t) lo, st, launches);
+    if (rc != CUIPM_OK) return rc;
+    CK(cudaMemcpyAsync(sol + so, s->d_sol + so, sizeof(double) * s->P.sol_stride * n, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(info + lo, s->d_info + lo, sizeof(cuipm_info) * n, cudaMemcpyDeviceToHost, st));
+    if (stat) CK(cudaMemcpyAsync(stat + to, s->d_stat + to, sizeof(double) * srow * n, cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(s->pipe_done[slot], st));
     return CUIPM_OK;
 }
 
@@ -240,12 +283,8 @@ extern "C" int cuipm_solve_device(cuipm_solver *s, int nbatch, const double *d_q
     CK(cudaSetDevice(s->device));
     s->last_launches = 0;
     if (nbatch == 0) return CUIPM_OK;
-    LaunchArgs a;
-    a.P = s->P; a.sd = s->d_sd; a.ipool = s->d_ipool; a.qp = d_qp; a.sol = d_sol; a.work = s->d_work; a.info = d_info;
-    a.stat = d_stat; a.o = *opts; a.nbatch = nbatch; a.seed = nullptr; a.sens = nullptr; a.adjoint = 0;
-    s->last_opts = *opts;
     CK(cudaEventRecord(s->ev0, s->stream));
-    rc = launch_batch(s, a, 0, 0, s->stream, &s->last_launches);
+    rc = launch_batch(s, launch_args(s, 0, nbatch, d_qp, d_sol, d_info, d_stat, opts), 0, 0, s->stream, &s->last_launches);
     if (rc != CUIPM_OK) return rc;
     CK(cudaEventRecord(s->ev1, s->stream));
     if (sync)
@@ -276,14 +315,7 @@ extern "C" int cuipm_solve_host_async(cuipm_solver *s, int nbatch, const double 
         if (rc != CUIPM_OK) return rc;
     }
     if (nbatch == 0) return CUIPM_OK;
-    const size_t stat_n = (size_t) nbatch * CUIPM_STAT_M * (opts->stat_max + 1);
-    if (stat && s->stat_cap < stat_n)
-    {
-        cudaFree(s->d_stat);
-        s->d_stat = nullptr;
-        CK(cudaMalloc(&s->d_stat, sizeof(double) * stat_n));
-        s->stat_cap = stat_n;
-    }
+    if (stat && !stat_buffer(s, (size_t) nbatch * CUIPM_STAT_M * (opts->stat_max + 1))) return CUIPM_ERR_CUDA;
     // Chunked pipeline: chunk c is copied in, solved and copied out on its own stream, so the H2D copy of the next chunk
     // (the batch is ~0.4 MB per QP) overlaps the solve of the previous ones; kernels of different chunks share the SMs.
     const int nchunk = nbatch >= 512 ? s->npipe : 1;
@@ -294,29 +326,12 @@ extern "C" int cuipm_solve_host_async(cuipm_solver *s, int nbatch, const double 
     {
         const int lo = c * per, n = std::min(per, nbatch - lo);
         if (n <= 0) break;
-        cudaStream_t st = s->pipe[c];
-        CK(cudaStreamWaitEvent(st, s->ev0, 0));
-        const size_t qo = s->P.qp_stride * (size_t) lo, so = s->P.sol_stride * (size_t) lo;
-        CK(cudaMemcpyAsync(s->d_qp + qo, qp + qo, sizeof(double) * s->P.qp_stride * n, cudaMemcpyHostToDevice, st));
-        if (opts->warm_start >= 1)
-            CK(cudaMemcpyAsync(s->d_sol + so, sol + so, sizeof(double) * s->P.sol_stride * n, cudaMemcpyHostToDevice, st));
-        LaunchArgs a;
-        a.P = s->P; a.sd = s->d_sd; a.ipool = s->d_ipool; a.qp = s->d_qp + qo; a.sol = s->d_sol + so;
-        a.work = s->d_work + s->P.work_stride * (size_t) lo; a.info = s->d_info + lo;
-        a.stat = stat ? s->d_stat + (size_t) lo * CUIPM_STAT_M * (opts->stat_max + 1) : nullptr;
-        a.o = *opts; a.nbatch = n; a.seed = nullptr; a.sens = nullptr; a.adjoint = 0;
-        rc = launch_batch(s, a, c, (size_t) lo, st, &nlaunch);
+        CK(cudaStreamWaitEvent(s->pipe[c], s->ev0, 0));
+        rc = enqueue_chunk(s, c, lo, n, qp, sol, info, stat, opts, &nlaunch);
         if (rc != CUIPM_OK) return rc;
-        CK(cudaMemcpyAsync(sol + so, s->d_sol + so, sizeof(double) * s->P.sol_stride * n, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(info + lo, s->d_info + lo, sizeof(cuipm_info) * n, cudaMemcpyDeviceToHost, st));
-        if (stat)
-            CK(cudaMemcpyAsync(stat + (size_t) lo * CUIPM_STAT_M * (opts->stat_max + 1), a.stat,
-                               sizeof(double) * (size_t) n * CUIPM_STAT_M * (opts->stat_max + 1), cudaMemcpyDeviceToHost, st));
-        CK(cudaEventRecord(s->pipe_done[c], st));
         CK(cudaStreamWaitEvent(s->stream, s->pipe_done[c], 0));
     }
     s->last_launches = nlaunch;
-    s->last_opts = *opts;
     CK(cudaEventRecord(s->ev1, s->stream));
     s->pending = 1;
     return CUIPM_OK;
@@ -337,24 +352,10 @@ extern "C" int cuipm_solve_host_chunk(cuipm_solver *s, int slot, int lo, int n, 
     if (rc != CUIPM_OK) return rc;
     CK(cudaSetDevice(s->device));
     if (n == 0) return CUIPM_OK;
-    cudaStream_t st = s->pipe[slot];
-    const size_t qo = s->P.qp_stride * (size_t) lo, so = s->P.sol_stride * (size_t) lo;
-    CK(cudaMemcpyAsync(s->d_qp + qo, qp + qo, sizeof(double) * s->P.qp_stride * n, cudaMemcpyHostToDevice, st));
-    if (opts->warm_start >= 1)
-        CK(cudaMemcpyAsync(s->d_sol + so, sol + so, sizeof(double) * s->P.sol_stride * n, cudaMemcpyHostToDevice, st));
-    LaunchArgs a;
-    a.P = s->P; a.sd = s->d_sd; a.ipool = s->d_ipool; a.qp = s->d_qp + qo; a.sol = s->d_sol + so;
-    a.work = s->d_work + s->P.work_stride * (size_t) lo; a.info = s->d_info + lo;
-    a.stat = nullptr;
-    a.o = *opts; a.nbatch = n; a.seed = nullptr; a.sens = nullptr; a.adjoint = 0;
     int nlaunch = 0;
-    rc = launch_batch(s, a, slot, (size_t) lo, st, &nlaunch);
+    rc = enqueue_chunk(s, slot, lo, n, qp, sol, info, nullptr, opts, &nlaunch);
     if (rc != CUIPM_OK) return rc;
-    CK(cudaMemcpyAsync(sol + so, s->d_sol + so, sizeof(double) * s->P.sol_stride * n, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(info + lo, s->d_info + lo, sizeof(cuipm_info) * n, cudaMemcpyDeviceToHost, st));
-    CK(cudaEventRecord(s->pipe_done[slot], st));
     s->last_launches = nlaunch;
-    s->last_opts = *opts;
     return CUIPM_OK;
 }
 
@@ -400,10 +401,8 @@ extern "C" int cuipm_sens_device(cuipm_solver *s, int nbatch, const double *d_qp
     CK(cudaSetDevice(s->device));
     s->last_launches = 0;
     if (nbatch == 0) return CUIPM_OK;
-    LaunchArgs a;
-    a.P = s->P; a.sd = s->d_sd; a.ipool = s->d_ipool; a.qp = d_qp; a.sol = nullptr; a.work = s->d_work; a.info = nullptr;
-    a.stat = nullptr; a.o = *opts; a.nbatch = nbatch; a.seed = d_seed; a.sens = d_sens; a.adjoint = adjoint != 0;
-    a.redo_list = nullptr; a.redo_count = nullptr;
+    LaunchArgs a = launch_args(s, 0, nbatch, d_qp, nullptr, nullptr, nullptr, opts);
+    a.seed = d_seed; a.sens = d_sens; a.adjoint = adjoint != 0;
     CK(cudaEventRecord(s->ev0, s->stream));
     rc = s->generic.sens(a, (void *) s->stream);
     if (rc != CUIPM_OK) return rc;

@@ -19,6 +19,9 @@ int smem_limit(const void *kernel, size_t *bytes);
 int set_dynamic_smem(const void *kernel, size_t bytes);
 // Sets the message "<what>: <CUDA error string of err (a cudaError_t)>" and returns CUIPM_ERR_CUDA.
 int cuda_error(const std::string &what, int err);
+// The solver's statistics buffer, grown to at least n doubles (the old one is freed after the solver's stream has drained);
+// null (+ message) if that fails.
+double *stat_buffer(cuipm_solver *s, size_t n);
 }  // namespace cuipm
 
 // CUDA runtime call in a function that returns a cuipm status: on failure, the message names the call

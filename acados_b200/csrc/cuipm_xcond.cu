@@ -19,13 +19,9 @@ struct cuipm_xcond
     int device = 0, max_batch = 0, N = 0, cond_N = 0;
     cuipm_reducer *red = nullptr;
     cuipm_condenser *cond = nullptr;
-    cuipm_solver *solver = nullptr;
+    cuipm_solver *solver = nullptr;                    // its device buffers hold the records, solutions and summaries it solves
     const cuipm_layout *lf = nullptr, *lr = nullptr;
-    cuipm_layout *lc = nullptr;                        // layout of the condensed records (owned; null without condensing)
-    double *d_full = nullptr, *d_red = nullptr, *d_cond = nullptr, *d_sol = nullptr, *d_sol_red = nullptr, *d_sol_full = nullptr;
-    double *d_stat = nullptr;                          // statistics tables, grown on demand
-    size_t stat_cap = 0;
-    cuipm_info *d_info = nullptr;
+    double *d_full = nullptr, *d_red = nullptr, *d_sol_red = nullptr, *d_sol_full = nullptr;   // d_red, d_sol_red: condensing only
     int lhs_valid = 0;
 };
 
@@ -38,9 +34,7 @@ extern "C" void cuipm_xcond_destroy(cuipm_xcond *x)
     if (x->solver) cuipm_destroy(x->solver);
     if (x->cond) cuipm_condenser_destroy(x->cond);
     if (x->red) cuipm_reducer_destroy(x->red);
-    if (x->lc) cuipm_layout_destroy(x->lc);
-    cudaFree(x->d_full); cudaFree(x->d_red); cudaFree(x->d_cond); cudaFree(x->d_sol); cudaFree(x->d_sol_red); cudaFree(x->d_sol_full);
-    cudaFree(x->d_stat); cudaFree(x->d_info);
+    cudaFree(x->d_full); cudaFree(x->d_red); cudaFree(x->d_sol_red); cudaFree(x->d_sol_full);
     delete x;
 }
 
@@ -61,21 +55,15 @@ extern "C" cuipm_xcond *cuipm_xcond_create(const cuipm_shape *full, int nbxe0, c
         x->cond = cuipm_condenser_create(ssh, x->cond_N, device);
         if (!x->cond) return fail();
         ssh = cuipm_condenser_condensed_shape(x->cond);
-        x->lc = cuipm_layout_create(ssh);
     }
-    x->solver = cuipm_create(ssh, max_batch, device);
+    x->solver = cuipm_create(ssh, max_batch, device);   // zeroes its solutions: the first warm start starts from zeros
     if (!x->solver) return fail();
-    const cuipm_layout *ls = x->lc ? x->lc : x->lr;
     const size_t nb = (size_t) max_batch;
     if (cudaSetDevice(device) != cudaSuccess
         || cudaMalloc(&x->d_full, sizeof(double) * x->lf->qp_stride * nb) != cudaSuccess
-        || cudaMalloc(&x->d_red, sizeof(double) * x->lr->qp_stride * nb) != cudaSuccess
-        || (x->lc && cudaMalloc(&x->d_cond, sizeof(double) * x->lc->qp_stride * nb) != cudaSuccess)
-        || cudaMalloc(&x->d_sol, sizeof(double) * ls->sol_stride * nb) != cudaSuccess
-        || (x->lc && cudaMalloc(&x->d_sol_red, sizeof(double) * x->lr->sol_stride * nb) != cudaSuccess)
-        || cudaMalloc(&x->d_sol_full, sizeof(double) * x->lf->sol_stride * nb) != cudaSuccess
-        || cudaMalloc(&x->d_info, sizeof(cuipm_info) * nb) != cudaSuccess
-        || cudaMemset(x->d_sol, 0, sizeof(double) * ls->sol_stride * nb) != cudaSuccess)   // the first warm start starts from zeros
+        || (x->cond && cudaMalloc(&x->d_red, sizeof(double) * x->lr->qp_stride * nb) != cudaSuccess)
+        || (x->cond && cudaMalloc(&x->d_sol_red, sizeof(double) * x->lr->sol_stride * nb) != cudaSuccess)
+        || cudaMalloc(&x->d_sol_full, sizeof(double) * x->lf->sol_stride * nb) != cudaSuccess)
     {
         set_error("cuipm_xcond_create: device allocation failed (no CPU fallback)");
         return fail();
@@ -88,7 +76,8 @@ extern "C" int cuipm_xcond_cond_N(const cuipm_xcond *x) { return x ? x->cond_N :
 extern "C" cuipm_solver *cuipm_xcond_solver(cuipm_xcond *x) { return x ? x->solver : nullptr; }
 
 // mode 0: one pass; 1: preparation phase only (reduce + condense_lhs); 2: feedback phase (reduce + condense_rhs + solve + ...)
-// d_sol holds the solver's (reduced or condensed) solution of the previous call: warm starts (warm_start >= 2) start from it
+// The solver's own buffers hold its records (reduced, or condensed: condense_rhs refreshes those condense_lhs left there) and its
+// solution of the previous call, from which warm starts (warm_start >= 2) start.
 static int chain(cuipm_xcond *x, int mode, int nbatch, const double *qp_full, double *sol_full, cuipm_info *info, double *stat,
                  const cuipm_opts *opts)
 {
@@ -100,38 +89,33 @@ static int chain(cuipm_xcond *x, int mode, int nbatch, const double *qp_full, do
     if (mode == 2 && x->cond && x->lhs_valid < nbatch) { set_error("cuipm_xcond_condense_rhs_and_solve_host: call cuipm_xcond_condense_lhs_host first"); return CUIPM_ERR_INVALID; }
     if (nbatch == 0) return CUIPM_OK;
     CK(cudaSetDevice(x->device));
-    cudaStream_t st = (cudaStream_t) cuipm_stream(x->solver);
+    cuipm_solver *s = x->solver;
+    cudaStream_t st = (cudaStream_t) cuipm_stream(s);
+    double *d_qp = cuipm_device_qp_buffer(s), *d_sol = cuipm_device_sol_buffer(s);
+    cuipm_info *d_info = cuipm_device_info_buffer(s);
     const size_t stat_n = stat ? (size_t) nbatch * CUIPM_STAT_M * (opts->stat_max + 1) : 0;
-    if (x->stat_cap < stat_n)
-    {
-        CK(cudaStreamSynchronize(st));
-        cudaFree(x->d_stat);
-        x->d_stat = nullptr;
-        CK(cudaMalloc(&x->d_stat, sizeof(double) * stat_n));
-        x->stat_cap = stat_n;
-    }
+    double *d_stat = stat ? stat_buffer(s, stat_n) : nullptr;
+    if (stat && !d_stat) return CUIPM_ERR_CUDA;
     CK(cudaMemcpyAsync(x->d_full, qp_full, sizeof(double) * x->lf->qp_stride * (size_t) nbatch, cudaMemcpyHostToDevice, st));
-    RCX(cuipm_reduce_device(x->red, nbatch, x->d_full, x->d_red, st));
-    const double *d_qp = x->d_red;
+    RCX(cuipm_reduce_device(x->red, nbatch, x->d_full, x->cond ? x->d_red : d_qp, st));
     if (x->cond)
     {
-        if (mode == 2) RCX(cuipm_condense_rhs_device(x->cond, nbatch, x->d_red, x->d_cond, st));
-        else RCX(cuipm_condense_lhs_device(x->cond, nbatch, x->d_red, x->d_cond, st));
+        if (mode == 2) RCX(cuipm_condense_rhs_device(x->cond, nbatch, x->d_red, d_qp, st));
+        else RCX(cuipm_condense_lhs_device(x->cond, nbatch, x->d_red, d_qp, st));
         if (mode != 2) x->lhs_valid = nbatch;
-        d_qp = x->d_cond;
     }
     if (mode == 1) { CK(cudaStreamSynchronize(st)); return CUIPM_OK; }
-    RCX(cuipm_solve_device(x->solver, nbatch, d_qp, x->d_sol, x->d_info, stat ? x->d_stat : nullptr, opts, 0));
-    const double *d_sr = x->d_sol;
+    RCX(cuipm_solve_device(s, nbatch, d_qp, d_sol, d_info, d_stat, opts, 0));
+    const double *d_sr = d_sol;
     if (x->cond)
     {
-        RCX(cuipm_expand_device(x->cond, nbatch, x->d_red, x->d_sol, x->d_sol_red, st));
+        RCX(cuipm_expand_device(x->cond, nbatch, x->d_red, d_sol, x->d_sol_red, st));
         d_sr = x->d_sol_red;
     }
     RCX(cuipm_restore_device(x->red, nbatch, x->d_full, d_sr, x->d_sol_full, opts->lam_min, opts->t_min, st));
     CK(cudaMemcpyAsync(sol_full, x->d_sol_full, sizeof(double) * x->lf->sol_stride * (size_t) nbatch, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(info, x->d_info, sizeof(cuipm_info) * (size_t) nbatch, cudaMemcpyDeviceToHost, st));
-    if (stat) CK(cudaMemcpyAsync(stat, x->d_stat, sizeof(double) * stat_n, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(info, d_info, sizeof(cuipm_info) * (size_t) nbatch, cudaMemcpyDeviceToHost, st));
+    if (stat) CK(cudaMemcpyAsync(stat, d_stat, sizeof(double) * stat_n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     return CUIPM_OK;
 }

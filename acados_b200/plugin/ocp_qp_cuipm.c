@@ -94,6 +94,25 @@ static acados_size_t idx_pool_len(const ocp_qp_dims *dims)
     return n;
 }
 
+/* shape of `in`, its idxb / idxs_rev (-1 on stages without slacks) copied into pool with per-stage pointers idxb_p / rev_p */
+static cuipm_shape shape_from_in(const ocp_qp_in *in, int *pool, int **idxb_p, int **rev_p)
+{
+    const ocp_qp_dims *d = in->dim;
+    int o = 0;
+    for (int k = 0; k <= d->N; k++)
+    {
+        idxb_p[k] = pool + o;
+        for (int i = 0; i < d->nb[k]; i++) pool[o++] = in->idxb[k][i];
+        rev_p[k] = pool + o;
+        for (int i = 0; i < d->nb[k] + d->ng[k]; i++) pool[o++] = d->ns[k] > 0 ? in->idxs_rev[k][i] : -1;
+    }
+    cuipm_shape sh;
+    shape_from_dims(d, &sh);
+    sh.idxb = (const int *const *) idxb_p;
+    sh.idxs_rev = (const int *const *) rev_p;
+    return sh;
+}
+
 acados_size_t ocp_qp_cuipm_memory_calculate_size(void *config_, void *dims_, void *opts_)
 {
     ocp_qp_dims *dims = dims_;
@@ -191,20 +210,12 @@ static void ensure_solver(ocp_qp_cuipm_memory *mem, ocp_qp_cuipm_opts *opts, con
     if (mem->solver && mem->max_batch >= nbatch && same_structure(mem, in)) return;
     if (mem->solver) cuipm_destroy(mem->solver);
     const ocp_qp_dims *d = in->dim;
-    int N = d->N, o = 0;
-    for (int k = 0; k <= N; k++)
+    for (int k = 0; k <= d->N; k++)
     {
         int *di = mem->dims_i + 5 * k;
         di[0] = d->nx[k]; di[1] = d->nu[k]; di[2] = d->nb[k]; di[3] = d->ng[k]; di[4] = d->ns[k];
-        mem->idxb_p[k] = mem->idx_pool + o;
-        for (int i = 0; i < d->nb[k]; i++) mem->idx_pool[o++] = in->idxb[k][i];
-        mem->idxs_rev_p[k] = mem->idx_pool + o;
-        for (int i = 0; i < d->nb[k] + d->ng[k]; i++) mem->idx_pool[o++] = d->ns[k] > 0 ? in->idxs_rev[k][i] : -1;
     }
-    cuipm_shape sh;
-    shape_from_dims(d, &sh);
-    sh.idxb = (const int *const *) mem->idxb_p;
-    sh.idxs_rev = (const int *const *) mem->idxs_rev_p;
+    cuipm_shape sh = shape_from_in(in, mem->idx_pool, mem->idxb_p, mem->idxs_rev_p);
     mem->solver = cuipm_create(&sh, nbatch, opts->device);
     mem->max_batch = nbatch;
     if (!mem->solver)
@@ -273,6 +284,28 @@ static int acados_status(int hpipm_status)
         case CUIPM_INCONS_EQ: return ACADOS_INFEASIBLE;
         default: return ACADOS_UNKNOWN;
     }
+}
+
+/* QP i of a batch back into its struct: solution, iteration count, acados status (status_out, if given) */
+static void hand_back(int i, const double *sol, const cuipm_info *infos, const cuipm_layout *l, ocp_qp_in **qp_in, ocp_qp_out **qp_out, int *status_out)
+{
+    unpack_sol(sol + l->sol_stride * (size_t) i, qp_in[i]->dim, l, qp_out[i]);
+    qp_info *info = qp_out[i]->misc;
+    info->interface_time = 0; info->num_iter = infos[i].iter; info->t_computed = 1;
+    if (status_out) status_out[i] = acados_status(infos[i].status);
+}
+
+/* the batch's wall-clock time t split evenly over its QPs' qp_info; returns the batch's worst acados status (its first failure) */
+static int batch_result(int n, ocp_qp_out **qp_out, const cuipm_info *infos, double t)
+{
+    int worst = ACADOS_SUCCESS;
+    for (int i = 0; i < n; i++)
+    {
+        qp_info *info = qp_out[i]->misc;
+        info->solve_QP_time = t / n; info->total_time = t / n;
+        if (worst == ACADOS_SUCCESS) worst = acados_status(infos[i].status);
+    }
+    return worst;
 }
 
 /************************************************
@@ -357,6 +390,26 @@ static int pack_threads(void)
     return nt;
 }
 
+/* page-locked staging of the batched entries (the plugin's raw memory is pageable and sized for one QP): records and summaries */
+static void staging_free(double **qp, double **sol, cuipm_info **info, int *cap)
+{
+    cuipm_host_free(*qp); cuipm_host_free(*sol); cuipm_host_free(*info);
+    *qp = *sol = NULL; *info = NULL; *cap = 0;
+}
+
+/* grows the staging to n QPs of layout l; 0 if an allocation failed (cuipm_last_error() says why) */
+static int staging_grow(const cuipm_layout *l, int n, double **qp, double **sol, cuipm_info **info, int *cap)
+{
+    if (*cap >= n) return 1;
+    staging_free(qp, sol, info, cap);
+    *qp = cuipm_host_alloc(sizeof(double) * l->qp_stride * (size_t) n);
+    *sol = cuipm_host_alloc(sizeof(double) * l->sol_stride * (size_t) n);
+    *info = cuipm_host_alloc(sizeof(cuipm_info) * (size_t) n);
+    if (!*qp || !*sol || !*info) return 0;
+    *cap = n;
+    return 1;
+}
+
 int ocp_qp_cuipm_batch_solve(void *config_, int n, ocp_qp_in **qp_in, ocp_qp_out **qp_out, void *opts_, void *mem_, int *status_out)
 {
     ocp_qp_cuipm_opts *opts = opts_;
@@ -366,17 +419,7 @@ int ocp_qp_cuipm_batch_solve(void *config_, int n, ocp_qp_in **qp_in, ocp_qp_out
     acados_tic(&timer);
     ensure_solver(mem, opts, qp_in[0], n);
     const cuipm_layout *l = cuipm_get_layout(mem->solver);
-    /* batch staging buffers: page-locked, owned by the memory object (the raw memory handed to the plugin is sized for one QP
-     * and pageable); grown when a larger batch arrives */
-    if (mem->b_cap < n)
-    {
-        cuipm_host_free(mem->b_qp); cuipm_host_free(mem->b_sol); cuipm_host_free(mem->b_info);
-        mem->b_qp = (double *) cuipm_host_alloc(sizeof(double) * l->qp_stride * (size_t) n);
-        mem->b_sol = (double *) cuipm_host_alloc(sizeof(double) * l->sol_stride * (size_t) n);
-        mem->b_info = (cuipm_info *) cuipm_host_alloc(sizeof(cuipm_info) * (size_t) n);
-        mem->b_cap = n;
-        if (!mem->b_qp || !mem->b_sol || !mem->b_info) { printf("\nerror: ocp_qp_cuipm_batch_solve: %s\n", cuipm_last_error()); exit(1); }
-    }
+    if (!staging_grow(l, n, &mem->b_qp, &mem->b_sol, &mem->b_info, &mem->b_cap)) { printf("\nerror: ocp_qp_cuipm_batch_solve: %s\n", cuipm_last_error()); exit(1); }
     double *qp = mem->b_qp, *sol = mem->b_sol;
     cuipm_info *infos = mem->b_info;
     /* Pipeline over chunks, two parallel regions in all (a region per chunk costs a barrier of the whole thread team each, which
@@ -414,8 +457,6 @@ int ocp_qp_cuipm_batch_solve(void *config_, int n, ocp_qp_in **qp_in, ocp_qp_out
         }
     }
     if (rc_all != CUIPM_OK) { printf("\nerror: ocp_qp_cuipm_batch_solve: %s\n", cuipm_last_error()); exit(1); }
-    int worst = ACADOS_SUCCESS;
-    double t_solve = 0.0;
     next = 0;
 #pragma omp parallel num_threads(nthr)
     {
@@ -432,24 +473,11 @@ int ocp_qp_cuipm_batch_solve(void *config_, int n, ocp_qp_in **qp_in, ocp_qp_out
                 if (cuipm_wait_chunk(mem->solver, c) != CUIPM_OK) { printf("\nerror: ocp_qp_cuipm_batch_solve: %s\n", cuipm_last_error()); exit(1); }
                 waited = c;
             }
-            unpack_sol(sol + l->sol_stride * (size_t) i, qp_in[i]->dim, l, qp_out[i]);
-            qp_info *info = qp_out[i]->misc;
-            info->interface_time = 0;
-            info->num_iter = infos[i].iter; info->t_computed = 1;
-            if (status_out) status_out[i] = acados_status(infos[i].status);
+            hand_back(i, sol, infos, l, qp_in, qp_out, status_out);
         }
     }
-    t_solve = acados_toc(&timer);
-    for (int i = 0; i < n; i++)
-    {
-        qp_info *info = qp_out[i]->misc;
-        info->solve_QP_time = t_solve / n; info->total_time = t_solve / n;
-    }
-    for (int i = 0; i < n; i++)
-    {
-        int st = acados_status(infos[i].status);
-        if (st != ACADOS_SUCCESS && worst == ACADOS_SUCCESS) worst = st;
-    }
+    const double t_solve = acados_toc(&timer);
+    const int worst = batch_result(n, qp_out, infos, t_solve);
     mem->info = infos[n - 1]; mem->status = infos[n - 1].status; mem->iter = infos[n - 1].iter; mem->time_qp_solver_call = t_solve;
     return worst;
 }
@@ -461,17 +489,17 @@ int ocp_qp_cuipm_batch_solve(void *config_, int n, ocp_qp_in **qp_in, ocp_qp_out
 struct ocp_qp_cuipm_xcond_batch
 {
     cuipm_xcond *x;
-    int n_max, N;
     int *pool, **idxb_p, **rev_p;
     double *b_qp, *b_sol;
     cuipm_info *b_info;
+    int b_cap;                  /* n_max of create: the most QPs a call may pass */
 };
 
 void ocp_qp_cuipm_xcond_batch_destroy(ocp_qp_cuipm_xcond_batch *c)
 {
     if (!c) return;
     if (c->x) cuipm_xcond_destroy(c->x);
-    cuipm_host_free(c->b_qp); cuipm_host_free(c->b_sol); cuipm_host_free(c->b_info);
+    staging_free(&c->b_qp, &c->b_sol, &c->b_info, &c->b_cap);
     free(c->pool); free(c->idxb_p); free(c->rev_p);
     free(c);
 }
@@ -479,37 +507,24 @@ void ocp_qp_cuipm_xcond_batch_destroy(ocp_qp_cuipm_xcond_batch *c)
 ocp_qp_cuipm_xcond_batch *ocp_qp_cuipm_xcond_batch_create(ocp_qp_in *in, int n_max, int cond_N, int device)
 {
     const ocp_qp_dims *d = in->dim;
-    const int N = d->N;
     if (d->nbue[0] > 0 || d->nge[0] > 0)
     {
         printf("\nerror: ocp_qp_cuipm_xcond_batch_create: only state-bound equalities at stage 0 are eliminated on the device\n");
         return NULL;
     }
     ocp_qp_cuipm_xcond_batch *c = calloc(1, sizeof(*c));
-    c->n_max = n_max; c->N = N;
     c->pool = calloc(idx_pool_len(d) + 1, sizeof(int));
-    c->idxb_p = calloc(N + 1, sizeof(int *));
-    c->rev_p = calloc(N + 1, sizeof(int *));
-    int o = 0;
-    for (int k = 0; k <= N; k++)
-    {
-        c->idxb_p[k] = c->pool + o;
-        for (int i = 0; i < d->nb[k]; i++) c->pool[o++] = in->idxb[k][i];
-        c->rev_p[k] = c->pool + o;
-        for (int i = 0; i < d->nb[k] + d->ng[k]; i++) c->pool[o++] = d->ns[k] > 0 ? in->idxs_rev[k][i] : -1;
-    }
-    cuipm_shape sh;
-    shape_from_dims(d, &sh);
-    sh.idxb = (const int *const *) c->idxb_p;
-    sh.idxs_rev = (const int *const *) c->rev_p;
+    c->idxb_p = calloc(d->N + 1, sizeof(int *));
+    c->rev_p = calloc(d->N + 1, sizeof(int *));
+    cuipm_shape sh = shape_from_in(in, c->pool, c->idxb_p, c->rev_p);
     /* equalities of stage 0: positions within [bu, bx, g] (d_ocp_qp.idxe, hpipm_d_ocp_qp.h:68) = positions in the bound list */
     c->x = cuipm_xcond_create(&sh, d->nbxe[0], in->idxe[0], cond_N, n_max, device);
-    if (!c->x) { printf("\nerror: ocp_qp_cuipm_xcond_batch_create: %s\n", cuipm_last_error()); ocp_qp_cuipm_xcond_batch_destroy(c); return NULL; }
-    const cuipm_layout *l = cuipm_xcond_full_layout(c->x);
-    c->b_qp = cuipm_host_alloc(sizeof(double) * l->qp_stride * (size_t) n_max);
-    c->b_sol = cuipm_host_alloc(sizeof(double) * l->sol_stride * (size_t) n_max);
-    c->b_info = cuipm_host_alloc(sizeof(cuipm_info) * (size_t) n_max);
-    if (!c->b_qp || !c->b_sol || !c->b_info) { printf("\nerror: ocp_qp_cuipm_xcond_batch_create: %s\n", cuipm_last_error()); ocp_qp_cuipm_xcond_batch_destroy(c); return NULL; }
+    if (!c->x || !staging_grow(cuipm_xcond_full_layout(c->x), n_max, &c->b_qp, &c->b_sol, &c->b_info, &c->b_cap))
+    {
+        printf("\nerror: ocp_qp_cuipm_xcond_batch_create: %s\n", cuipm_last_error());
+        ocp_qp_cuipm_xcond_batch_destroy(c);
+        return NULL;
+    }
     return c;
 }
 
@@ -517,7 +532,7 @@ int ocp_qp_cuipm_xcond_batch_solve(ocp_qp_cuipm_xcond_batch *c, int n, ocp_qp_in
                                    int *status_out)
 {
     ocp_qp_cuipm_opts *opts = opts_;
-    if (!c || n < 0 || n > c->n_max) { printf("\nerror: ocp_qp_cuipm_xcond_batch_solve: bad arguments\n"); exit(1); }
+    if (!c || n < 0 || n > c->b_cap) { printf("\nerror: ocp_qp_cuipm_xcond_batch_solve: bad arguments\n"); exit(1); }
     if (n == 0) return ACADOS_SUCCESS;
     acados_timer timer;
     acados_tic(&timer);
@@ -533,32 +548,23 @@ int ocp_qp_cuipm_xcond_batch_solve(ocp_qp_cuipm_xcond_batch *c, int n, ocp_qp_in
     if (phase == 1) return ACADOS_SUCCESS;
     const double t_solve = acados_toc(&timer);
 #pragma omp parallel for schedule(static) num_threads(nthr)
-    for (int i = 0; i < n; i++)
-    {
-        unpack_sol(c->b_sol + l->sol_stride * (size_t) i, qp_in[i]->dim, l, qp_out[i]);
-        qp_info *info = qp_out[i]->misc;
-        info->solve_QP_time = t_solve / n; info->interface_time = 0; info->total_time = t_solve / n;
-        info->num_iter = c->b_info[i].iter; info->t_computed = 1;
-        if (status_out) status_out[i] = acados_status(c->b_info[i].status);
-    }
-    int worst = ACADOS_SUCCESS;
-    for (int i = 0; i < n; i++)
-    {
-        int st = acados_status(c->b_info[i].status);
-        if (st != ACADOS_SUCCESS && worst == ACADOS_SUCCESS) worst = st;
-    }
-    return worst;
+    for (int i = 0; i < n; i++) hand_back(i, c->b_sol, c->b_info, l, qp_in, qp_out, status_out);
+    return batch_result(n, qp_out, c->b_info, t_solve);
+}
+
+/* drops the device solver and the batch staging, rebuilt on the next evaluate (ocp_qp_hpipm_memory_reset re-assigns its workspace) */
+static void release(ocp_qp_cuipm_memory *mem)
+{
+    if (mem->solver) cuipm_destroy(mem->solver);
+    mem->solver = NULL;
+    mem->max_batch = 0;
+    staging_free(&mem->b_qp, &mem->b_sol, &mem->b_info, &mem->b_cap);
 }
 
 void ocp_qp_cuipm_memory_reset(void *config_, void *qp_in_, void *qp_out_, void *opts_, void *mem_, void *work_)
 {
     ocp_qp_cuipm_memory *mem = mem_;
-    /* drop the device state; it is rebuilt on the next evaluate (ocp_qp_hpipm_memory_reset re-assigns its workspace) */
-    if (mem->solver) cuipm_destroy(mem->solver);
-    mem->solver = NULL;
-    mem->max_batch = 0;
-    cuipm_host_free(mem->b_qp); cuipm_host_free(mem->b_sol); cuipm_host_free(mem->b_info);
-    mem->b_qp = mem->b_sol = NULL; mem->b_info = NULL; mem->b_cap = 0;
+    release(mem);
     mem->status = 0;
     mem->iter = 0;
 }
@@ -631,14 +637,7 @@ void ocp_qp_cuipm_eval_adj_sens(void *config_, void *qp_in, void *seed, void *qp
 
 void ocp_qp_cuipm_terminate(void *config_, void *mem_, void *work_)
 {
-    ocp_qp_cuipm_memory *mem = mem_;
-    if (mem && mem->solver) cuipm_destroy(mem->solver);
-    if (mem)
-    {
-        mem->solver = NULL;
-        cuipm_host_free(mem->b_qp); cuipm_host_free(mem->b_sol); cuipm_host_free(mem->b_info);
-        mem->b_qp = mem->b_sol = NULL; mem->b_info = NULL; mem->b_cap = 0;
-    }
+    if (mem_) release(mem_);
 }
 
 void ocp_qp_cuipm_config_initialize_default(void *config_)

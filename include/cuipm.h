@@ -278,7 +278,9 @@ cuipm_xcond *cuipm_xcond_create(const cuipm_shape *full, int nbxe0, const int *i
 void cuipm_xcond_destroy(cuipm_xcond *x);
 const cuipm_layout *cuipm_xcond_full_layout(const cuipm_xcond *x);
 int cuipm_xcond_cond_N(const cuipm_xcond *x);
-cuipm_solver *cuipm_xcond_solver(cuipm_xcond *x);      /* the solver of the reduced / condensed shape (statistics, getters); owned by x */
+/* The solver of the reduced / condensed shape (statistics, getters, sensitivities); owned by x.  Its device buffers hold the
+ * reduced or condensed records and solutions of the last call. */
+cuipm_solver *cuipm_xcond_solver(cuipm_xcond *x);
 int cuipm_xcond_solve_host(cuipm_xcond *x, int nbatch, const double *qp_full, double *sol_full, cuipm_info *info, double *stat,
                            const cuipm_opts *opts);
 int cuipm_xcond_condense_lhs_host(cuipm_xcond *x, int nbatch, const double *qp_full);
