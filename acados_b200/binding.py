@@ -64,6 +64,18 @@ INFO_DTYPE = np.dtype([("status", np.int32), ("iter", np.int32), ("res_max", np.
                       align=True)
 assert INFO_DTYPE.itemsize == C.sizeof(CuipmInfo)
 
+# enum cuipm_field: the per-field sources of cuipm_xcond_assemble_device, under AcadosOcpQp's field names
+FIELD_IDS = {f: i for i, f in enumerate(("A", "B", "b", "Q", "R", "S", "q", "r", "lbu", "ubu", "lbx", "ubx", "C", "D", "lg", "ug",
+                                         "Zl", "Zu", "zl", "zu", "lls", "lus", "lbu_mask", "ubu_mask", "lbx_mask", "ubx_mask",
+                                         "lg_mask", "ug_mask", "lls_mask", "lus_mask"))}
+
+
+class CuipmSrc(C.Structure):
+    """Mirror of ``struct cuipm_src``: one field of one stage, element (r, c) of QP q at ptr[q*s_batch + r*s_row + c*s_col]."""
+    _fields_ = [("field", C.c_int), ("stage", C.c_int), ("ptr", C.c_void_p), ("s_batch", C.c_longlong), ("s_row", C.c_longlong),
+                ("s_col", C.c_longlong)]
+
+
 _lib: Optional[C.CDLL] = None
 
 
@@ -145,6 +157,13 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         f.restype = ip
     lib.cuipm_xcond_condense_lhs_host.argtypes = [vp, ip, vp]
     lib.cuipm_xcond_condense_lhs_host.restype = ip
+    for f in (lib.cuipm_xcond_solve_device, lib.cuipm_xcond_condense_rhs_and_solve_device):
+        f.argtypes = [vp, ip, vp, vp, vp, vp, C.POINTER(CuipmOpts), ip]
+        f.restype = ip
+    lib.cuipm_xcond_condense_lhs_device.argtypes = [vp, ip, vp, ip]
+    lib.cuipm_xcond_condense_lhs_device.restype = ip
+    lib.cuipm_xcond_assemble_device.argtypes = [vp, ip, C.POINTER(CuipmSrc), ip, vp, ip]
+    lib.cuipm_xcond_assemble_device.restype = ip
     lib.cuipm_set_tuning.argtypes = [vp, C.c_char_p, ip]
     lib.cuipm_set_tuning.restype = ip
     lib.cuipm_last_handed_back.argtypes = [vp]
@@ -380,6 +399,33 @@ class CuipmXcond:
 
     def condense_rhs_and_solve(self, qp_full, opts: CuipmOpts, want_stat: bool = False):
         return self._solve(self.lib.cuipm_xcond_condense_rhs_and_solve_host, qp_full, opts, want_stat)
+
+    # device-buffer entries: device pointers, work enqueued on ``stream``, a synchronise only with sync=True
+    def solve_device(self, nbatch: int, d_qp: int, d_sol: int, d_info: int, opts: CuipmOpts, d_stat: int = 0, sync: bool = False):
+        self._check(self.lib.cuipm_xcond_solve_device(self.handle, nbatch, d_qp, d_sol, d_info, d_stat or None, C.byref(opts),
+                                                      1 if sync else 0))
+
+    def condense_lhs_device(self, nbatch: int, d_qp: int, sync: bool = False):
+        self._check(self.lib.cuipm_xcond_condense_lhs_device(self.handle, nbatch, d_qp, 1 if sync else 0))
+
+    def condense_rhs_and_solve_device(self, nbatch: int, d_qp: int, d_sol: int, d_info: int, opts: CuipmOpts, d_stat: int = 0,
+                                      sync: bool = False):
+        self._check(self.lib.cuipm_xcond_condense_rhs_and_solve_device(self.handle, nbatch, d_qp, d_sol, d_info, d_stat or None,
+                                                                       C.byref(opts), 1 if sync else 0))
+
+    def assemble_device(self, nbatch: int, src, nsrc: int, d_qp: int, sync: bool = False):
+        """Records of the full shape from per-field sources (a ``CuipmSrc`` array; include/cuipm.h)."""
+        self._check(self.lib.cuipm_xcond_assemble_device(self.handle, nbatch, src, nsrc, d_qp, 1 if sync else 0))
+
+    @property
+    def solver_handle(self) -> int:
+        """The inner ``cuipm_solver *`` (statistics, sensitivities: ``cuipm_xcond_solver``)."""
+        return self.lib.cuipm_xcond_solver(self.handle)
+
+    @property
+    def stream(self) -> int:
+        """The ``cudaStream_t`` the device entries enqueue on."""
+        return self.lib.cuipm_stream(self.solver_handle)
 
     @property
     def last_kernel_ms(self) -> float:

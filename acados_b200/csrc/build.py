@@ -12,8 +12,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 OUT = os.path.join(HERE, "libcuipm.so")
-SOURCES = ["cuipm_kernel.cu", "cuipm_fast.cu", "cuipm_api.cu", "cuipm_reduce.cu", "cuipm_condense.cu", "cuipm_xcond.cu", "cuipm_host.cpp"]
-HEADERS = ["cuipm_device.h", "cuipm_internal.h", "cuipm_plan.h", "cuipm_fast_core.h", "cuipm_condense_core.h", "cuipm_condense_plan.h", os.path.join(ROOT, "include", "cuipm.h")]
+SOURCES = ["cuipm_kernel.cu", "cuipm_fast.cu", "cuipm_api.cu", "cuipm_reduce.cu", "cuipm_condense.cu", "cuipm_xcond.cu", "cuipm_assemble.cu", "cuipm_host.cpp"]
+HEADERS = ["cuipm_device.h", "cuipm_internal.h", "cuipm_plan.h", "cuipm_fast_core.h", "cuipm_condense_core.h", "cuipm_condense_plan.h", "cuipm_assemble_core.h", os.path.join(ROOT, "include", "cuipm.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
          "-I" + os.path.join(ROOT, "include"), "-I" + HERE]

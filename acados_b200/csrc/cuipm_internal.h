@@ -24,6 +24,27 @@ int cuda_error(const std::string &what, int err);
 double *stat_buffer(cuipm_solver *s, size_t n);
 }  // namespace cuipm
 
+namespace cuipm_asm { struct Stage; }
+// the assembly's part of an xcond object (cuipm_assemble.cu): its stage table from the full shape; freed with its device tables
+int asm_init(cuipm_xcond *x, const cuipm_shape *full);
+void asm_free(cuipm_xcond *x);
+
+// the xcond object (cuipm_xcond.cu; cuipm_assemble.cu writes its records)
+struct cuipm_xcond
+{
+    int device = 0, max_batch = 0, cond_N = 0;
+    cuipm_reducer *red = nullptr;
+    cuipm_condenser *cond = nullptr;
+    cuipm_solver *solver = nullptr;                    // its device buffers hold the records, solutions and summaries it solves
+    const cuipm_layout *lf = nullptr, *lr = nullptr;
+    double *d_full = nullptr, *d_sol_full = nullptr;   // host entries only: allocated at the first one
+    double *d_red = nullptr, *d_sol_red = nullptr;     // condensing only
+    int lhs_valid = 0;
+    cuipm_asm::Stage *asm_st = nullptr;                // the assembly's stage table of the full shape (N+1 entries), no sources
+    void *d_asm = nullptr;                             // device copy of the assembly's tables
+    size_t asm_bytes = 0;
+};
+
 // CUDA runtime call in a function that returns a cuipm status: on failure, the message names the call
 #define CK(call) do { const cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuipm::cuda_error(#call, (int) e_); } while (0)
 

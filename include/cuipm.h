@@ -267,12 +267,19 @@ int cuipm_condense_rhs_device(cuipm_condenser *c, int nbatch, const double *d_qp
  * Reference: ocp_qp_xcond_solver (acados/ocp_qp/ocp_qp_xcond_solver.c:523-669): condensing module + QP solver + expansion,
  * evaluate() in one piece or split into condense_lhs (:591-627, preparation phase of SQP-RTI) and condense_rhs_and_solve
  * (:629-669, feedback phase).  `full` is the shape as the user poses it, idxe0 as for cuipm_reducer_create; cond_N in 1..N
- * (<= 0 or N: no block condensing).  Records of the full shape come from (page-locked) host memory, solutions of the full
- * shape, the per-QP summaries and, if `stat` is not NULL, the statistics tables (as for cuipm_solve_host) go back; the reduced /
- * condensed records, the prediction matrices of the lhs pass and all intermediate solutions live on the device.  With
- * warm_start >= 2 the solve starts from this object's previous solution in the reduced / condensed layout (zeros before the
- * first solve), as the reference runs its QP solver on the condensed solution of the previous call unless
- * initialize_next_xcond_qp_from_qp_out is set (ocp_qp_xcond_solver.c:554-569). */
+ * (<= 0 or N: no block condensing).  The reduced / condensed records, the prediction matrices of the lhs pass and all
+ * intermediate solutions live on the device.  With warm_start >= 2 the solve starts from this object's previous solution in the
+ * reduced / condensed layout (zeros before the first solve), as the reference runs its QP solver on the condensed solution of
+ * the previous call unless initialize_next_xcond_qp_from_qp_out is set (ocp_qp_xcond_solver.c:554-569).
+ *
+ * Two kinds of entry run the same device chain:
+ *   _host:   records of the full shape come from (page-locked) host memory; solutions of the full shape, the per-QP summaries
+ *            and, if `stat` is not NULL, the statistics tables (as for cuipm_solve_host) go back; synchronises.  The object
+ *            allocates its device copies of the records and solutions at the first host call.
+ *   _device: as cuipm_solve_device -- device pointers on the object's device, the work enqueued on the stream of
+ *            cuipm_xcond_solver(x) (cuipm_stream), a synchronise only if `sync` != 0.  The reducer and the restore read
+ *            d_qp_full in place: it must stay unchanged until the call's work has completed.  d_stat may be NULL, else it holds
+ *            nbatch x (stat_max+1) x CUIPM_STAT_M doubles. */
 typedef struct cuipm_xcond cuipm_xcond;
 cuipm_xcond *cuipm_xcond_create(const cuipm_shape *full, int nbxe0, const int *idxe0, int cond_N, int max_batch, int device);
 void cuipm_xcond_destroy(cuipm_xcond *x);
@@ -286,6 +293,40 @@ int cuipm_xcond_solve_host(cuipm_xcond *x, int nbatch, const double *qp_full, do
 int cuipm_xcond_condense_lhs_host(cuipm_xcond *x, int nbatch, const double *qp_full);
 int cuipm_xcond_condense_rhs_and_solve_host(cuipm_xcond *x, int nbatch, const double *qp_full, double *sol_full, cuipm_info *info,
                                             double *stat, const cuipm_opts *opts);
+int cuipm_xcond_solve_device(cuipm_xcond *x, int nbatch, const double *d_qp_full, double *d_sol_full, cuipm_info *d_info,
+                             double *d_stat, const cuipm_opts *opts, int sync);
+int cuipm_xcond_condense_lhs_device(cuipm_xcond *x, int nbatch, const double *d_qp_full, int sync);
+int cuipm_xcond_condense_rhs_and_solve_device(cuipm_xcond *x, int nbatch, const double *d_qp_full, double *d_sol_full,
+                                              cuipm_info *d_info, double *d_stat, const cuipm_opts *opts, int sync);
+
+/* ---- records of the full shape assembled on the device from per-field sources ------------------------------------------
+ * Fields carry the names and orientation of the reference's AcadosOcpQp.set (interfaces/acados_template/acados_template/
+ * acados_ocp_qp.py): A is nx_next x nx, B nx_next x nu, S nu x nx, C ng x nx, D ng x nu, Q nx x nx, R nu x nu; the others are
+ * vectors.  lbu / ubu are the first nbu bounds of idxb (the entries < nu), lbx / ubx the others. */
+enum cuipm_field {
+    CUIPM_F_A, CUIPM_F_B, CUIPM_F_b, CUIPM_F_Q, CUIPM_F_R, CUIPM_F_S, CUIPM_F_q, CUIPM_F_r,
+    CUIPM_F_lbu, CUIPM_F_ubu, CUIPM_F_lbx, CUIPM_F_ubx, CUIPM_F_C, CUIPM_F_D, CUIPM_F_lg, CUIPM_F_ug,
+    CUIPM_F_Zl, CUIPM_F_Zu, CUIPM_F_zl, CUIPM_F_zu, CUIPM_F_lls, CUIPM_F_lus,
+    CUIPM_F_lbu_mask, CUIPM_F_ubu_mask, CUIPM_F_lbx_mask, CUIPM_F_ubx_mask, CUIPM_F_lg_mask, CUIPM_F_ug_mask,
+    CUIPM_F_lls_mask, CUIPM_F_lus_mask,
+    CUIPM_F_COUNT
+};
+/* One field of one stage for every QP of the batch: element (r, c) of QP q is ptr[q*s_batch + r*s_row + c*s_col] (vectors:
+ * element r, s_col unused).  Strides are in doubles and >= 0; s_batch = 0 gives every QP the same value. */
+typedef struct cuipm_src {
+    int field, stage;
+    const double *ptr;
+    long long s_batch, s_row, s_col;
+} cuipm_src;
+/* Writes nbatch records of the full shape of x into d_qp_full (device memory, nbatch x qp_stride doubles of
+ * cuipm_xcond_full_layout) -- the bits the host packer writes for the same data: HPIPM's record conventions (BAt = [B'; A'],
+ * both triangles of RSQ, DCt = [D'; C'], d = [lbu, lbx, lg, -ubu, -ubx, -ug, lls, lus], masks in the same order), zeros for
+ * the padding and for every field without a source, ones for masks without one.  One kernel on the stream of
+ * cuipm_xcond_solver(x), after the source table (built on the host each call) has been copied there; a synchronise only if
+ * `sync` != 0.  A (field, stage) given twice, a field that does not exist at its stage (size 0 there: dynamics at N, slacks
+ * where ns = 0, ...), a negative stride or a null pointer returns CUIPM_ERR_INVALID before anything is enqueued.  The sources
+ * are read when the kernel runs. */
+int cuipm_xcond_assemble_device(cuipm_xcond *x, int nbatch, const cuipm_src *src, int nsrc, double *d_qp_full, int sync);
 
 /* Riccati quantities of the last factorisation (reference: ocp_qp_hpipm_solver_get, ocp_qp_hpipm.c:417-478).
  * field in {"P","p","K","k","Lr"}; copies column-major data of QP `iqp`, stage `stage` into `value`. */
