@@ -283,6 +283,8 @@ extern "C" int cuipm_solve_device(cuipm_solver *s, int nbatch, const double *d_q
     CK(cudaSetDevice(s->device));
     s->last_launches = 0;
     if (nbatch == 0) return CUIPM_OK;
+    rc = s->fast.clear_counts((void *) s->stream);
+    if (rc != CUIPM_OK) return rc;
     CK(cudaEventRecord(s->ev0, s->stream));
     rc = launch_batch(s, launch_args(s, 0, nbatch, d_qp, d_sol, d_info, d_stat, opts), 0, 0, s->stream, &s->last_launches);
     if (rc != CUIPM_OK) return rc;
@@ -321,6 +323,8 @@ extern "C" int cuipm_solve_host_async(cuipm_solver *s, int nbatch, const double 
     const int nchunk = nbatch >= 512 ? s->npipe : 1;
     int nlaunch = 0;
     const int per = (nbatch + nchunk - 1) / nchunk;
+    rc = s->fast.clear_counts((void *) s->stream);
+    if (rc != CUIPM_OK) return rc;
     CK(cudaEventRecord(s->ev0, s->stream));
     for (int c = 0; c < nchunk; c++)
     {

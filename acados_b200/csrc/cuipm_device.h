@@ -195,7 +195,11 @@ struct FastPath
     // are recorded after the repack and after the last throughput-kernel launch.  Sets a.redo_list / a.redo_count to the QPs
     // handed back and adds to *launches; leaves `a` as it is if the path does not take the batch.  Returns CUIPM_OK or an error.
     int enqueue(LaunchArgs &a, size_t lo, int slot, void *stream, int *launches, void *ev_repacked, void *ev_done);
-    // QPs handed back by the last batch or chunks (inst not null, the solver's streams idle); -1 on error
+    // Clears the hand-back counts of every slot on `stream`, ahead of a solve whose chunks are enqueued behind it on that stream
+    // (a solve with fewer chunks than the previous one would otherwise report the earlier solve's counts of the slots it leaves
+    // unused, and a solve the path does not take would report all of them).  No-op without an instance.
+    int clear_counts(void *stream);
+    // QPs handed back since the last clear_counts (inst not null, the solver's streams idle); -1 on error
     int handed_back() const;
     void destroy();
 };

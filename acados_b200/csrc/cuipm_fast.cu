@@ -304,6 +304,13 @@ int FastPath::enqueue(LaunchArgs &a, size_t lo, int slot, void *stream_, int *la
     return CUIPM_OK;
 }
 
+int FastPath::clear_counts(void *stream)
+{
+    if (!inst) return CUIPM_OK;
+    CK(cudaMemsetAsync(ctr, 0, sizeof(int) * 2 * nslot, (cudaStream_t) stream));
+    return CUIPM_OK;
+}
+
 int FastPath::handed_back() const
 {
     std::vector<int> h(2 * nslot);

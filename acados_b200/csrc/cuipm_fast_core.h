@@ -2063,7 +2063,8 @@ struct Ker
         if (A.o.lq_fact == 1)
         {
             // a Cholesky step that leaves a large residual in the linear system switches the solve to the LQ
-            // refactorisation (x_ocp_qp_ipm.c:2246-2346): cold path, generic kernel
+            // refactorisation (x_ocp_qp_ipm.c:2246-2346): cold path, generic kernel.  The reference's clause for a NaN
+            // g[0] under a zero norm has no counterpart: gmax_nan propagates a NaN of any entry, so aff_g is then NaN, never 0
             if (L.aff_g > 1e-5 || L.aff_bdm_large)
                 if (act) { hand_back(q, info); act = false; }
         }

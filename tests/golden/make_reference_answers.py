@@ -6,6 +6,10 @@ is not built:
   reference/lq_cases.npz  the near-singular instances of the LQ refactorisation (test_oracle_lq_refactorisation):
                           iteration counts, statuses, LQ counts, input trajectories (float64), the whole solution and the
                           per-iteration statistics (float32: they are compared to 1e-6 and 1e-4 relative).
+  reference/nonfinite.npz poisoned batches and the masked-infinity family of tests/test_nonfinite_data.py, each QP solved by
+                          its own reference object (test_nonfinite_data.reference_answers): iteration counts, statuses, input
+                          trajectories (float64), the whole solution (float32, NaN and inf kept) and a SHA-256 of the records
+                          solved; per-QP statuses and iteration counts of the reference's xcond path on the QPs as posed.
   python tests/golden/make_reference_answers.py
 """
 import os
@@ -46,3 +50,10 @@ for name, make in LQ_CASES.items():
                 name + "_stat": stat[:, :rows, :14].astype(np.float32)})
     print(name, "iters", info["iter"].tolist(), "lq", info["lq_count"].tolist())
 np.savez_compressed(os.path.join(OUT, "lq_cases.npz"), **out)
+
+from test_nonfinite_data import reference_answers  # noqa: E402
+
+out = reference_answers()
+for key in sorted(k for k in out if k.endswith("_status")):
+    print(key[:-7], "iters", out[key[:-7] + "_iter"].tolist(), "status", out[key].tolist())
+np.savez_compressed(os.path.join(OUT, "nonfinite.npz"), **out)
